@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — env agent-steps/s of the vectorised QuadSwarm env step on B200 (BASELINE.json metric).
+"""bench.py — env agent-steps/s of the vectorised QuadSwarm env step on H100 (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--config c2|c3|c4] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--config c2|c3|c4] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one control step (2 physics sub-steps + collisions + observations, auto-reset included) of every env
 of the workload.  Default workload = BASELINE.json configs[2] ("c3"): 8 drones x 4096 envs PER GPU (weak scaling),
@@ -47,19 +47,6 @@ CONFIGS = {
 }
 
 
-def measured_traffic(config):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the step kernel per launch, from the committed ncu --set full
-    capture of this workload (profiles/r01_traffic.json), or None."""
-    for name in ('r02_traffic.json', 'r01_traffic.json'):
-        try:
-            v = json.load(open(os.path.join(ROOT, 'profiles', name))).get(config, {}).get('dram_bytes_per_launch')
-            if v is not None:
-                return v
-        except Exception:
-            pass
-    return None
-
-
 def hbm_peak():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
@@ -67,7 +54,7 @@ def hbm_peak():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (not measured)'
 
 
 class ClockSampler:
@@ -301,7 +288,7 @@ def run_reference_arm(args):
 # ------------------------------------------------------------------------------------------
 # CUDA arm
 # ------------------------------------------------------------------------------------------
-L2_BYTES = 140e6          # rings are sized past this (B200 L2 = 126 MB)
+L2_BYTES = 60e6           # rings are sized past this (H100 L2 = 50 MB); a constant, so that the inputs never depend on the device
 
 
 class StepRunner:
@@ -352,18 +339,23 @@ class StepRunner:
         self.Kg = max(d for d in range(1, kg_max + 1) if K % d == 0) if K > kg_max else K
         if self.Kg < min(64, K):
             self.Kg = min(K, kg_max)
+        # K not a multiple of Kg: the last K % Kg steps of the timed window are one more graph, on ring slots of their own
+        self.tail = K % self.Kg
         need = int(np.ceil(L2_BYTES / (A * 16)))                            # slots until the ACTION ring alone exceeds L2
         self.NG = max(1, int(np.ceil(need / self.Kg)))
         while self.NG > 1 and self.NG * self.Kg * per_step > 8e9:           # bound the ring memory
             self.NG -= 1
         self.P = P = self.NG * self.Kg
+        slots = P + self.tail
         g = torch.Generator(device=dev)
         g.manual_seed(args.seed * 1000 + rank)
-        self.act = (torch.rand((P, E, self.N, 4), device=dev, generator=g) * 2 - 1).contiguous()
-        self.obs = torch.empty((P, E, self.N, D), device=dev)
-        self.rew = torch.empty((P, E, self.N), device=dev)
-        self.done = torch.empty((P, E, self.N), dtype=torch.uint8, device=dev)
+        self.act = (torch.rand((slots, E, self.N, 4), device=dev, generator=g) * 2 - 1).contiguous()
+        self.obs = torch.empty((slots, E, self.N, D), device=dev)
+        self.rew = torch.empty((slots, E, self.N), device=dev)
+        self.done = torch.empty((slots, E, self.N), dtype=torch.uint8, device=dev)
         self.counter = 0
+        self.last = 0                   # ring slot of the most recent step
+        self.tail_graph = None
         self.stream = torch.cuda.Stream(device=dev)
         self.stream.wait_stream(torch.cuda.current_stream(dev))       # set_state / the action ring were enqueued on the default stream
         self.graphs = []
@@ -380,14 +372,30 @@ class StepRunner:
                             self._one()
                     self.graphs.append(gr)
                 self.counter = 0
+                if self.tail:
+                    gr = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(gr, stream=self.stream):
+                        self.run_tail()                 # eager launches, captured
+                    self.tail_graph = gr
 
-    def _one(self):
-        k = self.counter % self.P
+    def _one(self, slot=None):
+        k = self.counter % self.P if slot is None else slot
         if self.wrapped:
             self.eng.wrap_step(self.act[k], obs_out=self.obs[k], rewards_out=self.rew[k], dones_out=self.done[k])
         else:
             self.eng.step(self.act[k], obs_out=self.obs[k], rewards_out=self.rew[k], dones_out=self.done[k])
-        self.counter += 1
+        self.last = k
+        if slot is None:
+            self.counter += 1
+
+    def run_tail(self):
+        """The self.tail steps on the tail slots: replayed from their graph once it exists."""
+        if self.tail_graph is not None:
+            self.tail_graph.replay()
+            self.last = self.P + self.tail - 1
+        else:
+            for i in range(self.tail):
+                self._one(self.P + i)
 
     def run(self, n):
         """n control steps on self.stream (call inside `with torch.cuda.stream(self.stream)`)."""
@@ -407,14 +415,15 @@ class StepRunner:
 
     def close(self):
         self.graphs = []
+        self.tail_graph = None
         self.eng.close()
 
 
-def time_blocks(torch, dist, runner, K, R, world, side=None, metrics=None, gather_every=100):
-    """R back-to-back blocks of exactly K control steps, each bracketed by its own pair of CUDA events on the launching
-    stream.  Returns the (start, end) event pairs.  The optional cross-GPU metrics gather (NCCL all-reduce of a small
-    vector every `gather_every` steps) runs on a side stream that only WAITS for the step stream — it is never an edge of
-    the step chain — and is joined after the last block."""
+def time_blocks(torch, dist, runner, sizes, world, side=None, metrics=None, gather_every=100):
+    """Back-to-back blocks of sizes[i] control steps, each bracketed by its own pair of CUDA events on the launching
+    stream; no untimed step runs between or after them.  Returns the (start, end) event pairs.  The optional cross-GPU
+    metrics gather (NCCL all-reduce of a small vector every `gather_every` steps) runs on a side stream that only WAITS for
+    the step stream — it is never an edge of the step chain — and is joined after the last block."""
     st = runner.stream
     pairs = []
     since = 0
@@ -424,21 +433,20 @@ def time_blocks(torch, dist, runner, K, R, world, side=None, metrics=None, gathe
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
-        for b in range(R):
+        for n in sizes:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(st)
-            runner.run(K)
+            runner.run(n) if n == runner.Kg else runner.run_tail()
             e1.record(st)
             pairs.append((e0, e1))
-            since += K
+            since += n
             if side is not None and since >= gather_every:
                 since = 0
                 side.wait_event(e1)
                 with torch.cuda.stream(side):
-                    metrics[0] = runner.rew[(runner.counter - 1) % runner.P].sum()
+                    metrics[0] = runner.rew[runner.last].sum()
                     metrics[1] += 1
                     dist.all_reduce(metrics[:1], async_op=True)
-            runner.align()                      # K > steps per graph: untimed steps up to the next graph boundary
         st.synchronize()
         if side is not None:
             side.synchronize()
@@ -456,8 +464,9 @@ def block_times(torch, dist, pairs, world, dev):
     return ms
 
 
-def measure_workload(torch, dist, name, args, local_rank, rank, world, K, target_s, clocks=None, side=None, metrics=None, wrapped=False):
-    """Device-resident agent-steps/s of one workload: R blocks of K chained step launches, median block."""
+def measure_workload(torch, dist, name, args, local_rank, rank, world, K, clocks=None, side=None, metrics=None, wrapped=False):
+    """Device-resident agent-steps/s of one workload: exactly K timed control steps (chained step launches) in blocks of
+    one CUDA graph each, median step time over the blocks."""
     cfg = CONFIGS[name]
     E = (args.envs if name == args.config and args.envs else cfg['E'])
     runner = StepRunner(torch, cfg, E, args, local_rank, rank, K, graph=not args.no_graph, stagger=not args.lockstep, wrapped=wrapped)
@@ -465,15 +474,11 @@ def measure_workload(torch, dist, name, args, local_rank, rank, world, K, target
     with torch.cuda.stream(runner.stream):
         runner.run(max(3, args.warmup))
         runner.align()
+        runner.run(runner.NG * runner.Kg if runner.graphs else 0)      # every graph of the timed window replayed once
+        runner.run_tail()
         runner.stream.synchronize()
-    # pilot blocks: estimate the block time, warm the graphs
-    evp = time_blocks(torch, dist, runner, K, 2, world)
-    est_ms = max(1e-3, evp[1][0].elapsed_time(evp[1][1]))
-    R = int(min(5000, max(1, np.ceil(target_s * 1e3 / est_ms))))
-    if world > 1:
-        t = torch.tensor([R], device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        R = int(t.item())
+    sizes = [runner.Kg] * (K // runner.Kg) + ([runner.tail] if runner.tail else [])
+    R = len(sizes)
     if side is not None:                       # NCCL's lazy channel / connection setup happens here, not in the window
         with torch.cuda.stream(side):
             metrics[0] = runner.rew[0].sum()
@@ -482,24 +487,42 @@ def measure_workload(torch, dist, name, args, local_rank, rank, world, K, target
     launches0 = runner.eng.launch_count
     if clocks is not None:
         clocks.start()
-    K_eff = K
-    pairs = time_blocks(torch, dist, runner, K, R, world, side=side, metrics=metrics)
+    pairs = time_blocks(torch, dist, runner, sizes, world, side=side, metrics=metrics)
     clk = clocks.stop() if clocks is not None else None
     ms = block_times(torch, dist, pairs, world, dev)
     if runner.eng.handover_timeouts:
         raise RuntimeError("a per-block hand-over between step grids timed out: results of this run are invalid")
-    med = float(np.median(ms))
+    step_ms = [m / n for m, n in zip(ms, sizes)]
     D, M, N, A = runner.D, runner.M, runner.N, runner.A
     b_alg = 292 + 4 * D + (8.0 * M / N if M else 0.0)
     peak, peak_src = hbm_peak()
-    launch_s = med * 1e-3 / K_eff
-    res = dict(runner=runner, med_ms=med, blocks=R, block_ms_min=float(np.min(ms)), block_ms_max=float(np.max(ms)),
-               us_per_step=launch_s * 1e6, value=world * A * K_eff / (med * 1e-3), b_alg=b_alg, D=D, M=M, N=N, A=A, E=E,
+    launch_s = float(np.median(step_ms)) * 1e-3
+    res = dict(runner=runner, blocks=R, block_steps=runner.Kg, step_ms_min=float(np.min(step_ms)), step_ms_max=float(np.max(step_ms)),
+               us_per_step=launch_s * 1e6, value=world * A / launch_s, b_alg=b_alg, D=D, M=M, N=N, A=A, E=E,
                frac=b_alg * A / launch_s / 1e9 / peak, achieved=b_alg * A / launch_s / 1e9, peak=peak, peak_src=peak_src,
                clk=clk, launches_host=runner.eng.launch_count - launches0, ring_slots=runner.P,
                ring_mb=dict(actions=runner.P * A * 16 / 1e6, observations=runner.P * A * D * 4 / 1e6), graphs=runner.NG,
                steps_per_graph=runner.Kg)
     return res
+
+
+DUMP_MAX_BYTES = 60_000_000           # under 64 MB with the .npy headers
+
+
+def dump_outputs(runner, out_dir):
+    """What the last timed step returned to its caller (observations, rewards, dones of every env of this GPU) as
+    float32 .npy files.  Above DUMP_MAX_BYTES a fixed, seeded sample of env rows is written, with their ids."""
+    k = runner.last
+    out = dict(obs=runner.obs[k], rewards=runner.rew[k], dones=runner.done[k])
+    out = {n: v.float().cpu().numpy() for n, v in out.items()}
+    row_bytes = sum(v[0].nbytes for v in out.values())
+    if runner.E * row_bytes > DUMP_MAX_BYTES:
+        keep = np.sort(np.random.RandomState(0).choice(runner.E, DUMP_MAX_BYTES // (row_bytes + 8), replace=False))
+        out = {n: v[keep] for n, v in out.items()}
+        out['env_ids'] = keep.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for n, v in out.items():
+        np.save(os.path.join(out_dir, f'{n}.npy'), v)
 
 
 def run_cuda_arm(args):
@@ -521,11 +544,13 @@ def run_cuda_arm(args):
     side = torch.cuda.Stream(device=dev) if world > 1 else None
     metrics = torch.zeros(64, device=dev) if world > 1 else None
     clocks = ClockSampler(local_rank) if rank == 0 else None
-    main = measure_workload(torch, dist, args.config, args, local_rank, rank, world, K, args.target_seconds, clocks=clocks,
+    main = measure_workload(torch, dist, args.config, args, local_rank, rank, world, K, clocks=clocks,
                             side=side, metrics=metrics, wrapped=args.wrapped_main)
     runner = main['runner']
     E, N, A, D, M = main['E'], main['N'], main['A'], main['D'], main['M']
     gathers = int(metrics[1].item()) if metrics is not None else 0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(runner, args.dump_outputs)
     runner.close()
     del runner
     torch.cuda.empty_cache()
@@ -658,7 +683,7 @@ def run_cuda_arm(args):
             del o, r, d_, acts
             # (a') the headline workload with the reference's default wrapper stack behind every step (csrc/qs_wrap.cuh)
             sub = argparse.Namespace(**vars(args))
-            m = measure_workload(torch, dist, args.config, sub, local_rank, rank, world, min(K, 2000), 0.15, wrapped=True)
+            m = measure_workload(torch, dist, args.config, sub, local_rank, rank, world, K, wrapped=True)
             agg = m['runner'].eng.wrap_read(reset=False)
             from quad_swarm_rl_b200 import _lib as L_
             extra['wrapped'] = {'us_per_step': m['us_per_step'], 'agent_steps_per_s': m['value'], 'vs_bare_step': m['us_per_step'] / main['us_per_step'],
@@ -676,14 +701,14 @@ def run_cuda_arm(args):
             for name in ('c2', 'c4', 'c5'):
                 if name == args.config:
                     continue
-                m = measure_workload(torch, dist, name, sub, local_rank, rank, world, min(K, 2000), 0.12)
+                m = measure_workload(torch, dist, name, sub, local_rank, rank, world, K)
                 per_cfg[name] = {'workload': CONFIGS[name]['desc'], 'us_per_step': m['us_per_step'], 'agent_steps_per_s': m['value'],
                                  'roofline_frac': m['frac'], 'alg_bytes_per_agent_step': m['b_alg'], 'blocks': m['blocks']}
                 m['runner'].close()
                 torch.cuda.empty_cache()
             extra['configs'] = per_cfg
             sub.envs = 4 * E
-            m = measure_workload(torch, dist, args.config, sub, local_rank, rank, world, min(K, 2000), 0.12)
+            m = measure_workload(torch, dist, args.config, sub, local_rank, rank, world, K)
             extra['large_batch'] = {'envs': 4 * E, 'agents': 4 * A, 'us_per_step': m['us_per_step'], 'agent_steps_per_s': m['value'],
                                     'roofline_frac': m['frac'],
                                     'note': 'same kernel, one launch per control step, 4x the envs of the headline workload'}
@@ -692,7 +717,7 @@ def run_cuda_arm(args):
             # BASELINE config c5 (8 drones x 4096 envs per GPU, obstacle-free, K=6) over all ranks, same protocol
             sub = argparse.Namespace(**vars(args))
             sub.envs = 0
-            m = measure_workload(torch, dist, 'c5', sub, local_rank, rank, world, min(K, 2000), 0.12, side=side, metrics=metrics)
+            m = measure_workload(torch, dist, 'c5', sub, local_rank, rank, world, K, side=side, metrics=metrics)
             extra['c5'] = {'workload': CONFIGS['c5']['desc'], 'n_gpus': world, 'envs_total': world * CONFIGS['c5']['E'],
                            'us_per_step': m['us_per_step'], 'agent_steps_per_s': m['value'], 'roofline_frac_per_gpu': m['frac']}
             m['runner'].close()
@@ -702,13 +727,13 @@ def run_cuda_arm(args):
         conf = bench_config(args, world)
         line = {
             'metric': 'env agent-steps/sec', 'value': main['value'], 'unit': 'agent-steps/s', 'n_gpus': world, 'steps': args.steps,
-            'warmup': args.warmup, 'ms_per_step': main['med_ms'] / K, 'higher_is_better': True, 'scaling': 'weak',
+            'warmup': args.warmup, 'ms_per_step': main['us_per_step'] * 1e-3, 'higher_is_better': True, 'scaling': 'weak',
             'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': conf,
-            'timing': {'protocol': (f'{main["blocks"]} back-to-back blocks of exactly {K} control steps, each block bracketed by CUDA events on the '
-                                    f'launching stream; value / ms_per_step are the MEDIAN block (max over ranks per block)'),
-                       'blocks': main['blocks'], 'block_ms_median': main['med_ms'], 'block_ms_min': main['block_ms_min'],
-                       'block_ms_max': main['block_ms_max'],
+            'timing': {'protocol': (f'exactly {K} timed control steps as {main["blocks"]} back-to-back blocks of up to {main["block_steps"]} steps, '
+                                    f'each block bracketed by CUDA events on the launching stream; value / ms_per_step are the MEDIAN '
+                                    f'step time of the blocks (max over ranks per block)'),
+                       'blocks': main['blocks'], 'step_ms_min': main['step_ms_min'], 'step_ms_max': main['step_ms_max'],
                        'episodes': ('generated on the device at every auto-reset' if dev_scn else 'host-generated tables, uploaded once'),
                        'auto_resets': ('envs start at staggered ticks: every control step carries E / (ep_len + 1) auto-resets' if not args.lockstep
                                        else 'envs in lock-step: all envs reset in the same step every ep_len + 1 steps'),
@@ -735,7 +760,7 @@ def run_cuda_arm(args):
                             'direction on this box'},
             'gpu_launches': int(K),
             'roofline': {'bound': 'hbm', 'achieved': main['achieved'], 'peak': main['peak'], 'unit': 'GB/s', 'frac': main['frac'],
-                         'traffic': measured_traffic(args.config) if E == cfg['E'] else None, 'peak_source': main['peak_src'],
+                         'peak_source': main['peak_src'],
                          'alg_bytes_per_agent_step': main['b_alg'], 'alg_bytes_per_launch': main['b_alg'] * A,
                          'launch_us': main['us_per_step']},
             'cpu_baseline': cpu,
@@ -760,11 +785,10 @@ def main():
     ap.add_argument('--wrapped-main', action='store_true', help='tuning: time the headline workload WITH the training wrappers (the line is then not the BASELINE metric)')
     ap.add_argument('--no-extras', action='store_true', help='skip the rollout / large-batch explanatory measurements')
     ap.add_argument('--lockstep', action='store_true', help='start all envs at tick 0 (all auto-resets fall into the same step)')
-    ap.add_argument('--target-seconds', type=float, default=0.5,
-                    help='repeat the K-step block until about this much time is measured (the clock sampler needs load)')
     ap.add_argument('--no-graph', action='store_true')
     ap.add_argument('--host-tables', action='store_true', help='use host-generated episode tables even where a device generator exists')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s outputs (rank 0) to DIR/*.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference_arm(args)

@@ -1,5 +1,5 @@
 /*
- * quadswarm.h — C ABI of the B200-native QuadSwarm vectorised environment step.
+ * quadswarm.h — C ABI of the H100-native QuadSwarm vectorised environment step.
  *
  * The reference (Zhehui-Huang/quad-swarm-rl) has NO FFI: its hot path is a Python object protocol
  * (SURVEY.md §8b).  This header is the boundary a binding would target; every entry point names the

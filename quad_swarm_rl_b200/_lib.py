@@ -1,6 +1,6 @@
 """ctypes binding of include/quadswarm.h (the C ABI of the CUDA env step).
 
-The shared library is built in-tree by `__graft_entry__.build()` (nvcc, sm_100a).  There is no CPU
+The shared library is built in-tree by `__graft_entry__.build()` (nvcc, sm_90a).  There is no CPU
 fallback: if the library is missing, loading fails loudly.
 """
 import ctypes as C

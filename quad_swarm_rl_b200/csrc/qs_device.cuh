@@ -1,4 +1,4 @@
-// Device-side building blocks of the QuadSwarm env step (sm_100a, fp32).
+// Device-side building blocks of the QuadSwarm env step (sm_90a, fp32).
 //
 // Each function states the reference behaviour it reproduces (file:line under
 // gym_art/quadrotor_multi/ of Zhehui-Huang/quad-swarm-rl); the float64 restatement the parity tests
@@ -14,8 +14,7 @@
 
 // Loads of mutable env state inside the step kernels.  QS_LD: always through L2 (rare paths).  ld_state<CG>: the hot
 // loads; CG = true in the step-kernel instantiations that hand over per block (qs_step.cuh: no kernel boundary, hence no
-// L1 invalidation, lies between the writer and the reader of a slot), plain cached loads otherwise (measured 0.1 us
-// faster per c3 step).
+// L1 invalidation, lies between the writer and the reader of a slot), plain cached loads otherwise (faster).
 #define QS_LD(ptr) __ldcg(ptr)
 
 namespace qs {

@@ -1,4 +1,4 @@
-// Keyed Philox4x32-10 draws for the QuadSwarm step kernels (sm_100a).
+// Keyed Philox4x32-10 draws for the QuadSwarm step kernels (sm_90a).
 //
 // Device twin of oracle/philox.py: both define the same function
 //   (seed, env, step_count, site, i, j, value_index) -> random value

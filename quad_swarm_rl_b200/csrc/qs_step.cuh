@@ -6,11 +6,11 @@
 // drone i.  All cross-drone traffic is __shfl_sync within the group; the env's pillar table is staged in
 // shared memory.  Follows QuadrotorEnvMulti.step, quadrotor_multi.py:413-724 (see DESIGN.md for the map).
 //
-// Shape of the code (measured, profiles/r01_*): at the benchmark sizes a B200 holds < 2 warps per SM
-// sub-partition, so the kernel is bound by instruction fetch and dependent-issue latency, not by HBM or
-// issue slots.  Hence: rolled loops (small instruction footprint), SFU approximations instead of the
-// branchy IEEE sqrt/div sequences, trigonometry-free contact code, and every rare path (contact
-// responses, random yaw, reset, re-drawn sensor noise) out of line.
+// Shape of the code: at the benchmark sizes the GPU holds < 2 warps per SM sub-partition, so the kernel
+// is bound by instruction fetch and dependent-issue latency, not by HBM or issue slots.  Hence: rolled
+// loops (small instruction footprint), SFU approximations instead of the branchy IEEE sqrt/div
+// sequences, trigonometry-free contact code, and every rare path (contact responses, random yaw, reset,
+// re-drawn sensor noise) out of line.
 #pragma once
 #include "qs_device.cuh"
 #include "qs_scenario.cuh"
@@ -439,8 +439,10 @@ __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key
     }
 }
 
+// 8 worker warps + the courier: c3 / c5 (1024 physics warps) keep the courier on 132 SMs.  One such CTA per SM (~130-170
+// registers); two per SM (<= 112 registers) spill, and on H100 were slower on c5, c2 and the wrapped step.
 #ifndef QS_LB
-#define QS_LB 256
+#define QS_LB 288
 #endif
 // named barriers of the split kernel (physics warp <-> observer warp, 64 threads).  Both warps use bar.sync: the
 // observer reaches barrier 1 first, the physics warp reaches barrier 2 first and has only its stores left to do.
@@ -477,7 +479,7 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, int parity) {
 }
 
 // running episode counter += v.  A reduction (RED.ADD, no return value): a load + store pair per counter put one L2
-// round trip per counter on the critical path of every warp with a discrete event (the debug-build timeline showed +3 us).
+// round trip per counter on the critical path of every warp with a discrete event.
 __device__ __forceinline__ void cnt_add(int32_t* c, int k, int v) { if (v != 0) atomicAdd(c + k, v); }
 
 // ---- per-block hand-over between consecutive step grids (pdl_mode 3) ----
@@ -655,7 +657,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
 
     // Programmatic dependent launch: wait here for the PREVIOUS step's grid to complete (and flush) before touching any
     // state; the trigger that lets the NEXT step's grid start launching is issued just before this grid's final stores
-    // (mode 2, default: hides ~0.3 us of launch latency per step; triggering at kernel start, mode 1, is 2 us SLOWER
+    // (mode 2, default: hides part of the launch latency of each step; triggering at kernel start, mode 1, is SLOWER
     // because the early grid competes for issue slots while it spins).  Without the launch attribute both are no-ops.
     if (HO) {
         // not chained: the stream predecessor may be a foreign kernel (it never triggers early, so this grid starts when
@@ -697,7 +699,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
     Phys ph;
     if (DYN) load_phys(st.dyn, valid ? a : 0, ph);
     // env-level words: issued together with the state loads, BEFORE the pillar staging below waits for its own loads (one
-    // L2 round trip for everything; the timeline of the debug build showed two serialized ones, 1.3 us of a 9.6 us step)
+    // L2 round trip for everything instead of two serialized ones)
     int4 ctr_raw = make_int4(0, 0, 0, 0);
     if (env_ok) ctr_raw = ld_state<HO>(st.env_ctr + env);
     // An env whose episode ends in this step (known from the tick just loaded) will need its next-episode record and its
@@ -1234,7 +1236,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
 
         // The env state is final here (only a goal event at site B below touches it again): its stores are issued before
         // the observation is built, so that the fence of the per-block hand-over at the end of the kernel finds them
-        // acknowledged instead of waiting a memory round trip for them (timeline: 1.4 -> 0.4 us after the last emit).
+        // acknowledged instead of waiting a memory round trip for them.
         if (!SPLIT && t == p.T - 1) {
             if (valid) store_agent(st, a, s, goal_dirty);
             if (valid && dsum_dirty) st.slots[SL_DIST_SUMS * st.a_pad + a] = dsum;

@@ -1,5 +1,5 @@
-// C ABI of the B200-native QuadSwarm env step (see include/quadswarm.h for the contract and the
-// reference interfaces each entry point replaces).  Build: nvcc -gencode arch=compute_100a,code=sm_100a.
+// C ABI of the H100-native QuadSwarm env step (see include/quadswarm.h for the contract and the
+// reference interfaces each entry point replaces).  Build: nvcc -gencode arch=compute_90a,code=sm_90a.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -358,15 +358,14 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
         return fail(QS_ERR_CUDA, "a per-block hand-over between step grids timed out earlier: the env state of this handle is "
                                  "not trustworthy any more (qs_handover_timeouts); destroy the handle");
     // split kernel: physics warp + observer warp per 32 drones (QS_SPLIT=0/1 at qs_create overrides the heuristic)
-    // Measured (profiles/r01_notes.md): splitting shortens one warp's dependency chain (32 envs: 6.9 -> 5.8 us per
-    // launch, 8 x 1024 envs: 8.05 -> 7.17 us) but adds work, so it only pays while the GPU has idle issue slots, i.e.
-    // up to about one physics warp per SM sub-partition (4 x 148 on B200).
+    // Splitting shortens one warp's dependency chain but adds work, so it only pays while the GPU has idle issue slots,
+    // i.e. up to about one physics warp per SM sub-partition (4 x the SM count).
     if (h->pregen_every > 0) {
         // next-episode records for the envs that consumed theirs (qs_pregen_kernel): every pregen_every step launches.  A
         // captured graph repeats exactly the launches of its capture: a short graph captured between two generator launches
         // and replayed forever never refills a record, and every auto-reset then generates its episode inside the step (same
-        // results; ~12 us per reset on c3, which the per-block hand-over mostly hides: 10.0 -> 10.4 us per step).  With
-        // QS_PREGEN_HEAD=1 every captured graph starts with a generator launch instead (costs ~10 us per replay).
+        // results; each such reset costs time, which the per-block hand-over mostly hides).  With QS_PREGEN_HEAD=1 every
+        // captured graph starts with a generator launch instead (which costs one more launch per replay).
         bool due = (h->since_pregen += p_in.T) >= h->pregen_every;
         static int head = -1;
         if (head < 0) { const char* e = getenv("QS_PREGEN_HEAD"); head = e ? atoi(e) : 0; }
@@ -385,7 +384,7 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     choose_obs_writeout(h, p, obs_in_device_memory);
     const long long phys_warps = ((long long)h->cfg.num_envs * h->NP + 31) / 32;
     // A chained handle whose batch gives every SM at least two warps steps faster in the balanced shape with a courier warp
-    // (below) than in the split shape: c2 (1024 envs x 8 drones) 7.03 -> 6.42 us per step.
+    // (below) than in the split shape.
     static int courier_env = -1;
     if (courier_env < 0) { const char* e = getenv("QS_COURIER"); courier_env = e ? atoi(e) : 1; }
     int sms = 0;
@@ -393,7 +392,7 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     const int wpc_all = (int)((phys_warps + sms - 1) / sms);
     const bool courier_shape = h->chained && courier_env && h->NP < 16 && h->st.dyn == nullptr && wpc_all >= 2 &&
                                (wpc_all + 1) * 32 <= QS_LB && ((wpc_all * 32) % h->NP) == 0;
-    const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4 * 148 && !courier_shape);
+    const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
     const bool split = want_split && p.obs_stage && h->NP > 1 && h->st.dyn == nullptr && !h->obst_random;
     // QS_BALANCE=1 (experiment): one CTA per SM, ceil(warps / SMs) warps each — every SM then holds the same number of warps
     // whatever the CTA scheduler does while two step grids overlap (the timeline of the debug build showed SMs with 6 CTAs
@@ -405,7 +404,6 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     bool balanced = false;
     if (balance && !split && h->NP < 16) {
         const int wpc = wpc_all;
-        // measured: c5 (8 x 4096, K = 6, staggered resets) 13.7 -> 10.0 us per step, c3 unchanged
         if (wpc >= 2 && wpc * 32 <= QS_LB && ((wpc * 32) % h->NP) == 0) { kBlock = wpc * 32; balanced = true; }
     }
     if (h->pdl_env == -2) {          // read once per handle
@@ -417,7 +415,7 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     // Balanced single-wave grids use the per-block hand-over with a COURIER warp (qs_step.cuh): one more warp per CTA that
     // carries no envs and does the hand-over's flag traffic — acquire of the predecessor's state word, early release of
     // this block's state (before the observation is built), the `done` word that orders the observation rows of consecutive
-    // steps.  Measured (profiles/r02_notes.md): c3 10.0 -> 8.5 us per step, c5 9.3 -> 8.6.  QS_COURIER=0 switches it off.
+    // steps.  QS_COURIER=0 switches it off.
     if (h->handover < 0 && balanced)          // decided before the first launch so that every grid of a chain has the same shape
         h->handover = pdl_env >= 0 ? (pdl_env == 3) : ((courier_env && kBlock + 32 <= QS_LB) || h->cfg.use_obstacles != 0);
     const bool courier = balanced && courier_env && h->handover == 1 && h->chained && h->st.dyn == nullptr && kBlock + 32 <= QS_LB;
@@ -433,17 +431,16 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     if (split) smem += (size_t)HAND_FLOATS * sizeof(float);
     // shared-memory footprint of a balanced CTA.  Without a courier warp: 120 KB, i.e. one CTA per SM and never two CTAs of
     // the same grid on one SM.  With it: 64 KB, so that the successor's CTA (whose block was released early) already runs on
-    // the SM while this one writes its observation rows; the register file limits an SM to two such CTAs anyway.
-    // Measured (c3 / c5, us per step): 120 KB 9.7 / 9.3, 100 KB 9.1 / 9.3, 70 KB 8.8 / 8.8, 48 KB 8.8 / 8.7.  QS_BALANCE_KB overrides.
+    // the SM while this one writes its observation rows, where registers allow (not the 9-warp CTAs, see QS_LB).
+    // QS_BALANCE_KB overrides.
     static int balance_kb = -1;
     if (balance_kb < 0) { const char* e = getenv("QS_BALANCE_KB"); balance_kb = e ? atoi(e) : 0; }
     const int pad_kb = balance_kb > 0 ? balance_kb : (courier ? 64 : 120);
     if (balanced && smem < (size_t)pad_kb * 1024) smem = (size_t)pad_kb * 1024;
     // Programmatic dependent launch between consecutive step grids (QS_PDL overrides; default -1 = choose per handle):
-    //   0 off; 1 grid-wide wait, trigger at kernel start (measured 2 us slower); 2 grid-wide wait, trigger before the final
-    //   stores (0.2-0.4 us faster per step than 0); 3 per-block hand-over, no grid-wide wait (qs_step.cuh).
-    // Measured (profiles/r01_notes.md): 3 wins when a step grid needs more than one wave of CTAs (c4: 29.3 -> 20.1 us,
-    // 16384 x 8 drones: 22.4 -> 19.8 us) and for the split shape (c2: 7.18 -> 6.99 us); for a single-wave grid whose
+    //   0 off; 1 grid-wide wait, trigger at kernel start (slower than 2); 2 grid-wide wait, trigger before the final
+    //   stores (faster than 0); 3 per-block hand-over, no grid-wide wait (qs_step.cuh).
+    // 3 wins when a step grid needs more than one wave of CTAs and for the split shape; for a single-wave grid whose
     // warps run in lock-step anyway (c3) its acquire / release costs what the hidden launch latency saves, so 2 stays.
     using KernelFn = void (*)(StepParams);
     const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
@@ -477,9 +474,9 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
             int per_sm = 0, sms = 0;
             QS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn_ho, kBlock, smem));
             QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-            // measured on c3 with envs resetting in different steps (round 2, profiles/r02_*): the reset of an env with a
-            // pillar table makes its block ~2 us late; with the grid-wide wait every step pays that (11.2 us), with the
-            // hand-over only the block's own chain does (10.2 us).  Lock-step envs: 9.2 vs 10.0 us (QS_PDL=2 selects it).
+            // with envs resetting in different steps, the reset of an env with a pillar table makes its block late; with
+            // the grid-wide wait every step pays that, with the hand-over only the block's own chain does.  Envs in
+            // lock-step favour the grid-wide wait (QS_PDL=2 selects it).
             h->handover = split || (long long)grid > (long long)per_sm * sms || h->cfg.use_obstacles != 0;
         }
     }
@@ -1006,7 +1003,7 @@ extern "C" int qs_rollout(QsHandle* h, int num_steps, const float* actions_dev, 
 }
 
 #ifndef QS_ZERO_COPY_DEFAULT
-#define QS_ZERO_COPY_DEFAULT true          // measured on c3: 148 -> 134 us per host-buffer step (profiles/r01_notes.md)
+#define QS_ZERO_COPY_DEFAULT true          // the kernel reads / writes the page-locked host buffers itself: no copy launches
 #endif
 // true when the host pointer is page-locked (cudaHostAlloc / cudaHostRegister): DMA can use it directly.  `dev` receives the
 // device alias of a mapped buffer (or null).  The last few answers are cached: a rollout worker passes the same buffers on

@@ -277,7 +277,7 @@ class _EnvBase:
         self.engine.close()
 
     def render(self, *a, **k):
-        raise NotImplementedError("rendering is out of scope of the B200 env step")
+        raise NotImplementedError("rendering is out of scope of the CUDA env step")
 
     # ---- infos
     def _reward_dicts(self, terms, coeff):

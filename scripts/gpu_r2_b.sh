@@ -9,7 +9,7 @@ run() { name=$1; shift; echo "== $name: $*" | tee -a gpurun_out/r2b_ab.txt; time
 import sys,json
 l=sys.stdin.read().strip()
 try:
-    d=json.loads(l); print(round(d['ms_per_step']*1e3,3),'us/step frac',round(d['roofline']['frac'],4),'blocks',d['timing']['blocks'],'min/max',round(d['timing']['block_ms_min'],4),round(d['timing']['block_ms_max'],4))
+    d=json.loads(l); print(round(d['ms_per_step']*1e3,3),'us/step frac',round(d['roofline']['frac'],4),'blocks',d['timing']['blocks'],'step min/max',round(d['timing']['step_ms_min']*1e3,3),round(d['timing']['step_ms_max']*1e3,3))
 except Exception as e: print('FAILED', l[-600:])
 " | tee -a gpurun_out/r2b_ab.txt; }
 run stag_wait python bench.py --steps 20 --warmup 5 $B

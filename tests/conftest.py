@@ -15,7 +15,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with `pytest -m gpu` on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with `pytest -m gpu` on an H100)")
     config.addinivalue_line("markers", "reference: needs the reference tree (/root/reference or oracle/_ref)")
 
 

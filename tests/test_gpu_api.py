@@ -274,14 +274,17 @@ def test_batched_env_mix_on_device_reports_scenario_names():
     env.close()
 
 
-@pytest.mark.parametrize('E,dev_scn', [(4096, 'o_random'), (300, 'o_static_same_goal')])
+@pytest.mark.parametrize('E,dev_scn', [(4096, 'o_random'), (None, 'o_random'), (300, 'o_static_same_goal')])
 def test_chained_step_grids_into_one_output_array(E, dev_scn):
     """Early hand-over of the courier warp: a block publishes its env state before its observation rows are written, and its
     successor starts on that.  When the caller gives every step the SAME output arrays, the rows of step t+1 must still land
     after those of step t (the `done` word, qs_step.cuh).  A graph of chained launches into one array must leave exactly what
-    stepping with a synchronisation after every launch leaves."""
+    stepping with a synchronisation after every launch leaves.  E = None: two physics warps per SM, a batch for which the
+    launcher picks the balanced shape with the courier warp whatever the SM count."""
     from quad_swarm_rl_b200.engine import QuadSwarmEngine
     T, N = 80, C3['num_agents']
+    if E is None:
+        E = 2 * (32 // N) * torch.cuda.get_device_properties(0).multi_processor_count
     mk = lambda: QuadSwarmEngine(num_envs=E, seed=4, ep_time=0.5, device_scenario=dev_scn, **C3)
     e1, e2 = mk(), mk()
     e1.set_chained(True); e2.set_chained(True)

@@ -1,4 +1,4 @@
-"""The C-ABI shared library: builds for sm_100a, loads without a GPU, exports every symbol include/quadswarm.h
+"""The C-ABI shared library: builds for sm_90a, loads without a GPU, exports every symbol include/quadswarm.h
 declares, and the ctypes mirror of QsConfig matches the C layout.  No compute calls (CPU-only)."""
 import ctypes
 import os
