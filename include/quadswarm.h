@@ -137,7 +137,7 @@ typedef struct QsConfig {
     int32_t use_obstacles;
     int32_t num_obstacles;           /* M = int(density * area) (quadrotor_multi.py:128) */
     int32_t use_downwash;
-    int32_t sense_noise;             /* 1 = 'default' (sensor_noise.py:70-76), 0 = bypass */
+    int32_t sense_noise;             /* 1 = 'default' (sensor_noise.py:70-76) or the set of qs_set_sensor_noise, 0 = bypass */
     float obst_size;                 /* pillar diameter */
     float room_dims[3];
     float ep_time;                   /* seconds; ep_len = int(ep_time / 0.01) (quadrotor_single.py:158) */
@@ -252,6 +252,36 @@ int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const float* rows_
  * collision test, the contact response and the 3x3 distance patch of that episode.  Needs a device-side obstacle scenario.
  * n_densities = n_sizes = 0 switches the randomisation off. */
 int qs_set_obstacle_randomization(QsHandle* h, const float* densities_host, int n_densities, const float* sizes_host, int n_sizes);
+
+/* Sensor-noise model — replaces SensorNoise(**sense_noise) (sensor_noise.py:69-110; quadrotor_single.py:236-247), one
+ * parameter set for every drone of the handle.  Per observation of a drone (get_state.py:6-72, numba path):
+ *   pos~ = pos + N(0, pos_norm_std) + U(-pos_unif_range, pos_unif_range), vel~ likewise,
+ *   omega~ = omega + N(0, gyro_noise_density),
+ *   R~ = quat2R(rot2quat(R) x quat_from_small_angle(theta)), theta = N(0, quat_norm_std) + U(-quat_unif_range, quat_unif_range).
+ * gyro_norm_std != 0 switches on the stateful gyro model (add_noise_to_omega, sensor_noise.py:221-231, dt = 0.005 s):
+ * omega~ = omega + b + gyro_random_walk N(0, 1) after b <- pi b + sigma_b N(0, 1), with one bias b per drone that starts at
+ * zero, is never reset and advances once per observation (a step draws up to three: its own, the re-draw after a contact
+ * response, the observation of an auto-reset).  The accelerometer parameters are not part of the struct: it is never observed.
+ * Every std and range must be finite and >= 0; gyro_bias_correlation_time > 0 when the gyro model is on.
+ * Call after qs_create and before the first qs_reset / qs_step; later calls fail with QS_ERR_INVALID_ARG (the reference sets
+ * the noise only in its constructor), as does a call on a handle whose QsConfig.sense_noise = 0.  Without a call the
+ * 'default' set (QsConfig.sense_noise = 1) is compiled into the kernels.  The custom model runs in the single-warp step shape
+ * with the grid-wide wait between steps. */
+typedef struct QsSensorNoise {
+    double pos_norm_std, pos_unif_range;
+    double vel_norm_std, vel_unif_range;
+    double quat_norm_std, quat_unif_range;
+    double gyro_noise_density;
+    double gyro_norm_std;                 /* != 0: stateful gyro bias */
+    double gyro_random_walk;
+    double gyro_bias_correlation_time;    /* seconds */
+} QsSensorNoise;
+int qs_set_sensor_noise(QsHandle* h, const QsSensorNoise* noise_host);
+
+/* Gyro bias of every drone, [E,N,3] floats (zeros while the gyro model is off; set fails then).  Part of the env state for
+ * snapshots: qs_get_state / qs_set_state do not carry it. */
+int qs_get_gyro_bias(QsHandle* h, float* bias_dev, void* stream);
+int qs_set_gyro_bias(QsHandle* h, const uint8_t* env_mask_dev, const float* bias_dev, void* stream);
 
 /* flag bits in agent_u32[.,0] */
 #define QS_FLAG_ON_FLOOR (1u << 0)

@@ -55,6 +55,12 @@ class QsConfig(C.Structure):
     ]
 
 
+class QsSensorNoise(C.Structure):
+    _fields_ = [(k, C.c_double) for k in ('pos_norm_std', 'pos_unif_range', 'vel_norm_std', 'vel_unif_range', 'quat_norm_std',
+                                           'quat_unif_range', 'gyro_noise_density', 'gyro_norm_std', 'gyro_random_walk',
+                                           'gyro_bias_correlation_time')]
+
+
 class QsWrapConfig(C.Structure):
     _fields_ = [('use_replay', C.c_int32), ('replay_buffer_size', C.c_int32), ('replay_prob', C.c_float),
                 ('replay_always_active', C.c_int32), ('reserved_', C.c_int32 * 4)]
@@ -91,6 +97,9 @@ EXPORTS = {
     'qs_set_chained': (C.c_int, [C.c_void_p, C.c_int]),
     'qs_set_obstacle_randomization': (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_float), C.c_int]),
     'qs_set_dynamics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    'qs_set_sensor_noise': (C.c_int, [C.c_void_p, C.POINTER(QsSensorNoise)]),
+    'qs_get_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    'qs_set_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_wrap_enable': (C.c_int, [C.c_void_p, C.POINTER(QsWrapConfig)]),
     'qs_wrap_step': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_wrap_apply': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

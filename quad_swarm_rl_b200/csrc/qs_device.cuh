@@ -93,6 +93,14 @@ struct DevState {
     float4* scn_f;          // [E][3]  formation size / layer distance / largest size / speed; centre 1; centre 2
 };
 
+// Custom sensor-noise model (qs_set_sensor_noise); read only by the NZ kernel instantiations.  bias_pi / bias_sigma are the
+// per-observation factors of add_noise_to_omega (sensor_noise.py:224-229), computed on the host in float64.
+struct NoiseModel {
+    float pos_std, pos_range, vel_std, vel_range, gyro_std, quat_std, quat_range;
+    float bias_pi, bias_sigma, random_walk;
+    int rot;                // quat_std or quat_range != 0: the observed rotation is perturbed
+};
+
 struct StepParams {
     alignas(64) unsigned char obs_map[128];     // CUtensorMap of the caller's observation array (obs_bulk == 1), see quadswarm.cu
     DevState st;
@@ -132,6 +140,9 @@ struct StepParams {
     int scenario, grid_l, grid_w;       // QS_SCENARIO_*, pillar grid cells along x / y
     int pdl_mode;                       // 0 off, 1 trigger dependents at kernel start, 2 trigger before the final stores,
                                         // 3 per-block hand-over: no grid-wide wait at all (see qs_step_kernel)
+    NoiseModel nz;                      // custom sensor-noise model (NZ instantiations)
+    float4* gyro_bias;                  // [A] xyz: gyro bias of the stateful gyro model (qs_set_sensor_noise), or null: model off
+                                        // (not in DevState: the scenario functions take that by value)
 };
 
 struct Agent {
@@ -550,9 +561,9 @@ __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], 
     s.flags = fl;
 }
 
-// rot2quat -> quat2R round trip of the observed rotation (sensor_noise.py:34-63,205-210; quad_utils.py:133-138);
-// the rotation-noise quaternion is the identity for the default noise set.
-__device__ __forceinline__ void observed_rotation(const float R[9], float out[9]) {
+// Observed rotation quat2R(rot2quat(R) x qt) (sensor_noise.py:34-63,205-210; quad_utils.py:133-159); qt is the
+// rotation-noise quaternion.  The default noise set has qt = identity and emits R directly instead (write_observation).
+__device__ __forceinline__ void observed_rotation(const float R[9], const float qt[4], float out[9]) {
     const float trace = R[0] + R[4] + R[8];
     float qw, qx, qy, qz;
     if (trace > 0.f) {
@@ -567,6 +578,13 @@ __device__ __forceinline__ void observed_rotation(const float R[9], float out[9]
     } else {
         const float S = fsqrt(1.0f + R[8] - R[0] - R[4]) * 2.f, iS = frcp(S);
         qw = (R[3] - R[1]) * iS; qx = (R[2] + R[6]) * iS; qy = (R[5] + R[7]) * iS; qz = 0.25f * S;
+    }
+    {   // quatXquat(quat, qt), quad_utils.py:148-159
+        const float w = qw * qt[0] - qx * qt[1] - qy * qt[2] - qz * qt[3];
+        const float x = qw * qt[1] + qx * qt[0] - qy * qt[3] + qz * qt[2];
+        const float y = qw * qt[2] + qx * qt[3] + qy * qt[0] - qz * qt[1];
+        const float z = qw * qt[3] - qx * qt[2] + qy * qt[1] + qz * qt[0];
+        qw = w; qx = x; qy = y; qz = z;
     }
     const float xx = 2.f * qx * qx, yy = 2.f * qy * qy, zz = 2.f * qz * qz;
     const float xy = 2.f * qx * qy, xz = 2.f * qx * qz, yz = 2.f * qy * qz;
@@ -591,6 +609,57 @@ __device__ __noinline__ Noise9 sensor_noise(RngKey key, uint32_t site, int i) {
     o.p[0] = POS_NOISE_STD * n[0]; o.p[1] = POS_NOISE_STD * n[1]; o.p[2] = POS_NOISE_STD * n[2];
     o.v[0] = VEL_NOISE_STD * n[3]; o.v[1] = VEL_NOISE_STD * n[4]; o.v[2] = VEL_NOISE_STD * n[5];
     o.w[0] = GYRO_NOISE_STD * n[6]; o.w[1] = GYRO_NOISE_STD * n[7]; o.w[2] = GYRO_NOISE_STD * n[8];
+    return o;
+}
+
+// One observation's noise under the custom model (qs_set_sensor_noise; add_noise_numba + add_noise_to_omega,
+// sensor_noise.py:172-231): offsets of position / velocity / gyro, the rotation-noise quaternion, and the gyro bias after this
+// observation.  kind = j of the draws (qs_rng.cuh, SITE_NOISE_*).  A block whose scale is zero is not drawn: the draws are
+// keyed, so skipping one changes no other.  Uniforms follow numba's low + (high - low) u.
+struct SensedNoise { Noise9 n; float q[4]; float3 bias; };
+__device__ __noinline__ SensedNoise sensor_noise_model(const NoiseModel& m, RngKey key, uint32_t kind, int i, float3 bias,
+                                                       bool gyro_model) {
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    SensedNoise o;
+    {
+        const float4 n = m.pos_std != 0.f ? rng_normal4(key, SITE_NOISE_N, i, kind, 0) : zero;
+        const float4 u = m.pos_range != 0.f ? rng_uniform4(key, SITE_NOISE_U, i, kind, 0) : zero;
+        const float lo = -m.pos_range, w = m.pos_range - lo;
+        o.n.p[0] = m.pos_std * n.x + (lo + w * u.x); o.n.p[1] = m.pos_std * n.y + (lo + w * u.y); o.n.p[2] = m.pos_std * n.z + (lo + w * u.z);
+    }
+    {
+        const float4 n = m.vel_std != 0.f ? rng_normal4(key, SITE_NOISE_N, i, kind, 1) : zero;
+        const float4 u = m.vel_range != 0.f ? rng_uniform4(key, SITE_NOISE_U, i, kind, 1) : zero;
+        const float lo = -m.vel_range, w = m.vel_range - lo;
+        o.n.v[0] = m.vel_std * n.x + (lo + w * u.x); o.n.v[1] = m.vel_std * n.y + (lo + w * u.y); o.n.v[2] = m.vel_std * n.z + (lo + w * u.z);
+    }
+    if (gyro_model) {
+        // b <- pi b + sigma_b N(0, 1); omega~ = omega + b + random_walk N(0, 1) (sensor_noise.py:228-231)
+        const float4 nb = rng_normal4(key, SITE_GYRO_BIAS, i, kind, 0), nw = rng_normal4(key, SITE_GYRO_BIAS, i, kind, 1);
+        bias.x = m.bias_pi * bias.x + m.bias_sigma * nb.x;
+        bias.y = m.bias_pi * bias.y + m.bias_sigma * nb.y;
+        bias.z = m.bias_pi * bias.z + m.bias_sigma * nb.z;
+        o.n.w[0] = bias.x + m.random_walk * nw.x; o.n.w[1] = bias.y + m.random_walk * nw.y; o.n.w[2] = bias.z + m.random_walk * nw.z;
+    } else {
+        const float4 n = m.gyro_std != 0.f ? rng_normal4(key, SITE_NOISE_N, i, kind, 2) : zero;
+        o.n.w[0] = m.gyro_std * n.x; o.n.w[1] = m.gyro_std * n.y; o.n.w[2] = m.gyro_std * n.z;
+    }
+    o.bias = bias;
+    o.q[0] = 1.f; o.q[1] = 0.f; o.q[2] = 0.f; o.q[3] = 0.f;
+    if (m.rot) {
+        const float4 n = m.quat_std != 0.f ? rng_normal4(key, SITE_NOISE_N, i, kind, 3) : zero;
+        const float4 u = m.quat_range != 0.f ? rng_uniform4(key, SITE_NOISE_U, i, kind, 2) : zero;
+        const float lo = -m.quat_range, w = m.quat_range - lo;
+        const float tx = m.quat_std * n.x + (lo + w * u.x), ty = m.quat_std * n.y + (lo + w * u.y), tz = m.quat_std * n.z + (lo + w * u.z);
+        // quat_from_small_angle, sensor_noise.py:11-23
+        const float q2 = (tx * tx + ty * ty + tz * tz) * 0.25f;
+        float qw, f;
+        if (q2 < 1.f) { qw = sqrtf(1.f - q2); f = 0.5f; }
+        else { qw = rsqrtf(1.f + q2); f = 0.5f * qw; }
+        const float qx = tx * f, qy = ty * f, qz = tz * f;
+        const float inv = rsqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
+        o.q[0] = qw * inv; o.q[1] = qx * inv; o.q[2] = qy * inv; o.q[3] = qz * inv;
+    }
     return o;
 }
 

@@ -39,6 +39,12 @@ enum Site : uint32_t {
     SITE_RESET_YAW_U = 14,  // (i)   uniforms v[k], k = rejection try            quadrotor_single.py:432-434
     SITE_SCENARIO_U = 15,   // (slot) env-level scenario generators
     SITE_HOT = 16,          // (i)   the draws every drone needs every step (OU + first sensor draw), compact layout below
+    // 17 = SITE_REPLAY_U (qs_wrap.cuh).  The custom sensor-noise model (qs_set_sensor_noise) draws full-precision values from
+    // its own sites (CPU twin: oracle/sensor_noise_oracle.py); j = which observation of the step: 0 its own, 1 the re-draw
+    // after a contact response, 2 an (auto-)reset.
+    SITE_NOISE_N = 18,      // (i,j) normals v0..2 pos, v4..6 vel, v8..10 gyro, v12..14 rotation angle   sensor_noise.py:241-256
+    SITE_NOISE_U = 19,      // (i,j) uniforms v0..2 pos, v4..6 vel, v8..10 rotation angle
+    SITE_GYRO_BIAS = 20,    // (i,j) normals v0..2 bias innovation, v4..6 random walk                    sensor_noise.py:221-231
 };
 
 constexpr int RESET_YAW_MAX_TRIES = 64;

@@ -67,7 +67,7 @@ __device__ __forceinline__ void write_observation(const StepParams& p, const Age
         const float px = s.pos[0] + nz.p[0], py = s.pos[1] + nz.p[1], pz = s.pos[2] + nz.p[2];
         // The reference observes quat2R(rot2quat(R)) (sensor_noise.py:205-210); with the default noise set the rotation
         // noise is exactly zero, the round trip is the identity up to rounding (<= 4e-16 in float64, SURVEY Appendix D-8),
-        // so R is emitted directly.  (`observed_rotation()` keeps the explicit round trip for reference.)
+        // so R is emitted directly.  The custom model's rotation noise (NZ) passes s.R = observed_rotation() in.
         const float* rot = s.R;
         if (valid) {
             row[0] = px - s.goal[0]; row[1] = py - s.goal[1]; row[2] = pz - s.goal[2];
@@ -585,8 +585,11 @@ __device__ __forceinline__ void hand_load(const float* hand, int lane, Agent& s,
 // chosen by the launcher when a step grid does not fit the GPU in one wave or the split shape is used.
 // DYN = true: per-drone physical constants (qs_set_dynamics; SURVEY 8f-4) instead of the compile-time Crazyflie set — only
 // instantiated for the single-warp shape with the grid-wide wait.
-template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false>
+// NZ = true: the custom sensor-noise model (qs_set_sensor_noise, p.nz) instead of the compile-time 'default' set; the gyro
+// bias (p.gyro_bias, when that model is on) rides in registers across the steps of a launch.  Same shape as DYN.
+template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false, bool NZ = false>
 __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const __grid_constant__ StepParams p) {
+    static_assert(!NZ || (!SPLIT && !HO), "the custom sensor-noise model runs in the single-warp shape with the grid-wide wait");
     extern __shared__ __align__(128) float2 s_obst[];
     __shared__ int s_late;          // courier launches: a block with a goal event behind the observation is released at its end
     __shared__ unsigned long long s_rows;      // courier launches: mbarrier, completes when the previous instance's observation rows are out
@@ -698,6 +701,13 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
     if (valid && role == 0) dsum = ld_state<HO>(st.slots + SL_DIST_SUMS * st.a_pad + a);
     Phys ph;
     if (DYN) load_phys(st.dyn, valid ? a : 0, ph);
+    const bool gyro_model = NZ && p.gyro_bias != nullptr;
+    float3 gb = make_float3(0.f, 0.f, 0.f);
+    if (gyro_model && valid) {
+        const float4 b = QS_LD(p.gyro_bias + a);
+        gb = make_float3(b.x, b.y, b.z);
+    }
+    float qt[4] = {1.f, 0.f, 0.f, 0.f};      // rotation-noise quaternion of the observation (NZ)
     // env-level words: issued together with the state loads, BEFORE the pillar staging below waits for its own loads (one
     // L2 round trip for everything instead of two serialized ones)
     int4 ctr_raw = make_int4(0, 0, 0, 0);
@@ -848,6 +858,12 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             nz.p[0] = on * POS_NOISE_STD * hn.sn[0]; nz.p[1] = on * POS_NOISE_STD * hn.sn[1]; nz.p[2] = on * POS_NOISE_STD * hn.sn[2];
             nz.v[0] = on * VEL_NOISE_STD * hn.sn[3]; nz.v[1] = on * VEL_NOISE_STD * hn.sn[4]; nz.v[2] = on * VEL_NOISE_STD * hn.sn[5];
             nz.w[0] = on * GYRO_NOISE_STD * hn.sn[6]; nz.w[1] = on * GYRO_NOISE_STD * hn.sn[7]; nz.w[2] = on * GYRO_NOISE_STD * hn.sn[8];
+            if (NZ) {
+                const SensedNoise sn = sensor_noise_model(p.nz, key, 0, i, gb, gyro_model);
+                nz = sn.n; gb = sn.bias;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) qt[k] = sn.q[k];
+            }
         }
 
         // ================= per-drone part: QuadrotorSingle._step, quadrotor_single.py:341-357 =================
@@ -1124,7 +1140,12 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             }
             if (kicked) {
                 s.flags |= QS_FLAG_KICKED;
-                if (!SPLIT && p.sense_noise) nz = sensor_noise(key, SITE_SENSOR1, i);      // fresh noise for every drone of the env (:598-599)
+                if (NZ) {
+                    const SensedNoise sn = sensor_noise_model(p.nz, key, 1, i, gb, gyro_model);
+                    nz = sn.n; gb = sn.bias;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) qt[k] = sn.q[k];
+                } else if (!SPLIT && p.sense_noise) nz = sensor_noise(key, SITE_SENSOR1, i);      // fresh noise for every drone of the env (:598-599)
             }
         }
 
@@ -1216,8 +1237,14 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
                 ctr.tick = 0;
                 ctr.episode_idx += 1;
                 goal_dirty = true;
+                if (NZ) {
+                    const SensedNoise sn = sensor_noise_model(p.nz, key, 2, i, gb, gyro_model);
+                    nz = sn.n; gb = sn.bias;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) qt[k] = sn.q[k];
+                }
                 if (!SPLIT) {
-                    if (p.sense_noise) nz = sensor_noise(key, SITE_SENSOR_RESET, i);
+                    if (!NZ && p.sense_noise) nz = sensor_noise(key, SITE_SENSOR_RESET, i);
                     dmin2 = min_pillar_dist2(p, s, s_obst_env);          // new pose, new pillar table
                 }
             }
@@ -1241,6 +1268,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             if (valid) store_agent(st, a, s, goal_dirty);
             if (valid && dsum_dirty) st.slots[SL_DIST_SUMS * st.a_pad + a] = dsum;
             if (env_ok && i == 0) st.env_ctr[env] = make_int4(ctr.tick, ctr.step_count + 1, ctr.svd_count, ctr.episode_idx);
+            if (gyro_model && valid) p.gyro_bias[a] = make_float4(gb.x, gb.y, gb.z, 0.f);
             stored_early = true;
             if (has_courier) {
                 // Early hand-over: the successor block only needs this block's env STATE, which is complete now; the
@@ -1259,6 +1287,13 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             bar_sync(3);                                               // observer is done with this step's hand-off
         } else if (!p.last_obs_only || t == p.T - 1) {
             float* gbase = p.obs + (p.last_obs_only ? 0 : (long long)t * A) * p.D;
+            // rotation noise (NZ): the observation is built with the perturbed rotation in s.R, which is restored after it
+            float R_true[9];
+            if (NZ && p.nz.rot) {
+#pragma unroll
+                for (int k = 0; k < 9; ++k) R_true[k] = s.R[k];
+                observed_rotation(R_true, qt, s.R);
+            }
             if (p.obs_stage) {
                 // rows go to the warp's shared-memory tile, then out through the bulk-copy engine (or coalesced vector stores)
                 const int slot = (lane / NP) * p.N + i;               // row of this drone inside the warp's tile
@@ -1273,6 +1308,10 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
                 __syncwarp();
             } else {
                 write_observation<NP>(p, s, nvel, nz, i, valid, s_obst_env, dmin2, gbase + a * p.D, obst_r);
+            }
+            if (NZ && p.nz.rot) {
+#pragma unroll
+                for (int k = 0; k < 9; ++k) s.R[k] = R_true[k];
             }
         }
         if (!SPLIT && dev_scn && __any_sync(0xffffffffu, scn_ev && !kicked)) {      // scenario tick, site B
@@ -1296,6 +1335,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         if (valid) store_agent(st, a, s, goal_dirty);
         if (valid && dsum_dirty) st.slots[SL_DIST_SUMS * st.a_pad + a] = dsum;
         if (env_ok && i == 0) st.env_ctr[env] = make_int4(ctr.tick, ctr.step_count, ctr.svd_count, ctr.episode_idx);
+        if (gyro_model && valid) p.gyro_bias[a] = make_float4(gb.x, gb.y, gb.z, 0.f);
     }
     if (!SPLIT && p.obs_bulk) {
         if (has_courier) bulk_drain_writes();         // ... and the `done` word promises that the rows are written
@@ -1311,8 +1351,8 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
     QS_TL(7);
 }
 
-// Explicit reset of the masked envs: QuadrotorEnvMulti.reset, quadrotor_multi.py:339-411.
-template <int NP>
+// Explicit reset of the masked envs: QuadrotorEnvMulti.reset, quadrotor_multi.py:339-411.  NZ: custom sensor-noise model.
+template <int NP, bool NZ = false>
 __global__ void __launch_bounds__(128) qs_reset_kernel(const __grid_constant__ StepParams p) {
     extern __shared__ __align__(128) float2 s_obst[];
     const DevState& st = p.st;
@@ -1374,10 +1414,22 @@ __global__ void __launch_bounds__(128) qs_reset_kernel(const __grid_constant__ S
     Noise9 nz;
 #pragma unroll
     for (int k = 0; k < 3; ++k) { nz.p[k] = 0.f; nz.v[k] = 0.f; nz.w[k] = 0.f; }
-    if (p.sense_noise) nz = sensor_noise(key, SITE_SENSOR_RESET, i);
+    if (NZ) {
+        const bool gyro_model = p.gyro_bias != nullptr;
+        float3 gb = make_float3(0.f, 0.f, 0.f);
+        if (gyro_model && valid) {
+            const float4 b = p.gyro_bias[a];
+            gb = make_float3(b.x, b.y, b.z);
+        }
+        const SensedNoise sn = sensor_noise_model(p.nz, key, 2, i, gb, gyro_model);
+        nz = sn.n;
+        if (gyro_model && valid) p.gyro_bias[a] = make_float4(sn.bias.x, sn.bias.y, sn.bias.z, 0.f);
+        if (valid) store_agent(st, a, s, true);
+        if (p.nz.rot) observed_rotation(s.R, sn.q, s.R);       // s.R is stored; only the observation sees the perturbed one
+    } else if (p.sense_noise) nz = sensor_noise(key, SITE_SENSOR_RESET, i);
     write_observation<NP>(p, s, nvel, nz, i, valid, s_obst_env, p.use_obst ? min_pillar_dist2(p, s, s_obst_env) : 1e4f,
                           p.obs + a * p.D, obst_r);
-    if (valid) store_agent(st, a, s, true);
+    if (!NZ && valid) store_agent(st, a, s, true);
 }
 
 // Generates, for every env that does not hold one yet, the record of its NEXT episode (see generate_episode above).  Launched

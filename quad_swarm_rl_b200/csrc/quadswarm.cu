@@ -1,5 +1,6 @@
 // C ABI of the H100-native QuadSwarm env step (see include/quadswarm.h for the contract and the
 // reference interfaces each entry point replaces).  Build: nvcc -gencode arch=compute_90a,code=sm_90a.
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -51,6 +52,10 @@ struct QsHandle {
     unsigned long long* tl;
     int tl_next;
 #endif
+    bool nz_on;           // qs_set_sensor_noise: the custom sensor-noise model (NZ kernels)
+    NoiseModel nz;
+    float4* gyro_bias;    // [A], allocated when the gyro bias model is on
+    bool started;         // a reset or step has been enqueued: the noise model is fixed from here on
     cudaStream_t last_stream;   // stream of the most recent asynchronous call of this handle
     bool async_pending;
     // staging for the *_host entry points (pinned host + device mirrors)
@@ -122,6 +127,8 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.obst_random = h->obst_random; p.n_obst_counts = h->n_obst_counts; p.n_obst_radii = h->n_obst_radii;
     for (int k = 0; k < QS_MAX_OBST_CHOICES; ++k) { p.obst_counts[k] = h->obst_counts[k]; p.obst_radii[k] = h->obst_radii[k]; }
     p.scenario = c.scenario; p.grid_l = c.obst_grid[0]; p.grid_w = c.obst_grid[1];
+    p.nz = h->nz;
+    p.gyro_bias = h->gyro_bias;
 }
 
 // Observation write-out mode of a step launch (qs_step.cuh, emit_observation_tile): the bulk-copy engine needs a 16-byte
@@ -390,10 +397,10 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     int sms = 0;
     QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
     const int wpc_all = (int)((phys_warps + sms - 1) / sms);
-    const bool courier_shape = h->chained && courier_env && h->NP < 16 && h->st.dyn == nullptr && wpc_all >= 2 &&
+    const bool courier_shape = h->chained && courier_env && h->NP < 16 && h->st.dyn == nullptr && !h->nz_on && wpc_all >= 2 &&
                                (wpc_all + 1) * 32 <= QS_LB && ((wpc_all * 32) % h->NP) == 0;
     const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
-    const bool split = want_split && p.obs_stage && h->NP > 1 && h->st.dyn == nullptr && !h->obst_random;
+    const bool split = want_split && p.obs_stage && h->NP > 1 && h->st.dyn == nullptr && !h->nz_on && !h->obst_random;
     // QS_BALANCE=1 (experiment): one CTA per SM, ceil(warps / SMs) warps each — every SM then holds the same number of warps
     // whatever the CTA scheduler does while two step grids overlap (the timeline of the debug build showed SMs with 6 CTAs
     // of 2 warps next to SMs with 2, and the step ends with the slowest block)
@@ -418,7 +425,8 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     // steps.  QS_COURIER=0 switches it off.
     if (h->handover < 0 && balanced)          // decided before the first launch so that every grid of a chain has the same shape
         h->handover = pdl_env >= 0 ? (pdl_env == 3) : ((courier_env && kBlock + 32 <= QS_LB) || h->cfg.use_obstacles != 0);
-    const bool courier = balanced && courier_env && h->handover == 1 && h->chained && h->st.dyn == nullptr && kBlock + 32 <= QS_LB;
+    const bool courier = balanced && courier_env && h->handover == 1 && h->chained && h->st.dyn == nullptr && !h->nz_on &&
+                         kBlock + 32 <= QS_LB;
     if (courier) kBlock += 32;
     p.courier = courier ? 1 : 0;
     const int work_warps = kBlock / 32 - (courier ? 1 : 0);
@@ -461,7 +469,17 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     });
     if (rc != QS_OK) return rc;
     KernelFn fn_dyn = nullptr;
-    if (h->st.dyn != nullptr) {           // per-drone physical constants: single-warp shape, grid-wide wait
+    if (h->nz_on) {                       // custom sensor-noise model (with or without per-drone constants): same shape as DYN
+        const bool dyn = h->st.dyn != nullptr;
+        dispatch_np(h->NP, [&](auto np) {
+            constexpr int NPv = decltype(np)::value;
+            fn_dyn = dyn ? (scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, true, true>
+                                : (KernelFn)qs_step_kernel<NPv, false, false, false, true, true>)
+                         : (scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, false, true>
+                                : (KernelFn)qs_step_kernel<NPv, false, false, false, false, true>);
+            return QS_OK;
+        });
+    } else if (h->st.dyn != nullptr) {    // per-drone physical constants: single-warp shape, grid-wide wait
         dispatch_np(h->NP, [&](auto np) {
             constexpr int NPv = decltype(np)::value;
             fn_dyn = scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, true> : (KernelFn)qs_step_kernel<NPv, false, false, false, true>;
@@ -513,6 +531,7 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     if (lerr != cudaSuccess) return fail(QS_ERR_CUDA, std::string("cudaLaunchKernelEx: ") + cudaGetErrorString(lerr));
     QS_CUDA(cudaGetLastError());
     h->launches += 1;
+    h->started = true;
     note_async(h, s, true);
     return QS_OK;
 }
@@ -541,12 +560,14 @@ static int launch_reset(QsHandle* h, const StepParams& p, cudaStream_t s) {
     const int grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
     const size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
     int rc = dispatch_np(h->NP, [&](auto np) {
-        qs_reset_kernel<decltype(np)::value><<<grid, kBlock, smem, s>>>(p);
+        if (h->nz_on) qs_reset_kernel<decltype(np)::value, true><<<grid, kBlock, smem, s>>>(p);
+        else qs_reset_kernel<decltype(np)::value><<<grid, kBlock, smem, s>>>(p);
         return QS_OK;
     });
     if (rc != QS_OK) return rc;
     QS_CUDA(cudaGetLastError());
     h->launches += 1;
+    h->started = true;
     note_async(h, s, false);
     return QS_OK;
 }
@@ -695,6 +716,7 @@ extern "C" int qs_destroy(QsHandle* h) {
     cudaFree(st.next_spawn); cudaFree(st.next_obst); cudaFree(st.stats_env); cudaFree(st.stats_agent);
     cudaFree(st.dyn); cudaFree(st.next_dyn); cudaFree(st.dyn_pending);
     cudaFree(st.scn_i); cudaFree(st.scn_f); cudaFree(st.ready); cudaFree(st.next_scn_i); cudaFree(st.next_scn_f); cudaFree(st.epi);
+    cudaFree(h->gyro_bias);
     cudaFree(h->d_actions); cudaFree(h->d_obs); cudaFree(h->d_rewards); cudaFree(h->d_terms); cudaFree(h->d_dones);
     cudaFree(h->d_mask);
     cudaFreeHost(h->h_actions); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rewards); cudaFreeHost(h->h_terms);
@@ -923,6 +945,77 @@ extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const f
     const long long n = A * (QS_DYN_ROW / 4);
     k_set_dynamics<<<blocks_for(n > E ? n : E), 256, 0, (cudaStream_t)stream>>>(st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev,
                                                                                (const float4*)rows_dev, at_next_reset ? 1 : 0);
+    QS_CUDA(cudaGetLastError());
+    h->launches += 1;
+    note_async(h, (cudaStream_t)stream, false);
+    return QS_OK;
+}
+
+extern "C" int qs_set_sensor_noise(QsHandle* h, const QsSensorNoise* sn) {
+    if (!h || !sn) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->started) return fail(QS_ERR_INVALID_ARG, "the sensor-noise model can only be set before the first reset or step");
+    if (!h->cfg.sense_noise) return fail(QS_ERR_INVALID_ARG, "sensor noise is bypassed on this handle (QsConfig.sense_noise = 0)");
+    const double v[10] = {sn->pos_norm_std, sn->pos_unif_range, sn->vel_norm_std, sn->vel_unif_range, sn->quat_norm_std,
+                          sn->quat_unif_range, sn->gyro_noise_density, sn->gyro_norm_std, sn->gyro_random_walk,
+                          sn->gyro_bias_correlation_time};
+    for (double x : v)
+        if (!(x >= 0.0) || !std::isfinite(x)) return fail(QS_ERR_INVALID_ARG, "sensor-noise parameters must be finite and >= 0");
+    const bool gyro_model = sn->gyro_norm_std != 0.0;
+    if (gyro_model && !(sn->gyro_bias_correlation_time > 0.0))
+        return fail(QS_ERR_INVALID_ARG, "gyro_bias_correlation_time must be > 0 when gyro_norm_std != 0");
+    NoiseModel m;
+    memset(&m, 0, sizeof(m));
+    m.pos_std = (float)sn->pos_norm_std; m.pos_range = (float)sn->pos_unif_range;
+    m.vel_std = (float)sn->vel_norm_std; m.vel_range = (float)sn->vel_unif_range;
+    m.gyro_std = (float)sn->gyro_noise_density;
+    m.quat_std = (float)sn->quat_norm_std; m.quat_range = (float)sn->quat_unif_range;
+    m.rot = (sn->quat_norm_std != 0.0 || sn->quat_unif_range != 0.0) ? 1 : 0;
+    if (gyro_model) {
+        // add_noise_to_omega, sensor_noise.py:224-229, in float64: exp(-2 dt / tau) - 1 as expm1 (no cancellation at large tau)
+        const double dt = (double)SIM_DT, tau = sn->gyro_bias_correlation_time;
+        const double sigma_g_d = sn->gyro_noise_density / std::sqrt(dt);
+        m.bias_pi = (float)std::exp(-dt / tau);
+        m.bias_sigma = (float)std::sqrt(-(sigma_g_d * sigma_g_d) * (tau / 2.0) * std::expm1(-2.0 * dt / tau));
+        m.random_walk = (float)sn->gyro_random_walk;
+        if (h->gyro_bias == nullptr) {
+            QS_CUDA(cudaSetDevice(h->device));
+            QS_ALLOC0(h->gyro_bias, sizeof(float4) * h->A);
+        }
+    } else if (h->gyro_bias != nullptr) {
+        cudaFree(h->gyro_bias);
+        h->gyro_bias = nullptr;
+    }
+    h->nz = m;
+    h->nz_on = true;
+    return QS_OK;
+}
+
+__global__ void k_gyro_bias(float4* bias, long long A, int N, const uint8_t* mask, float* out, const float* in) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= A) return;
+    if (out) {
+        const float4 b = bias ? bias[t] : make_float4(0.f, 0.f, 0.f, 0.f);
+        out[3 * t] = b.x; out[3 * t + 1] = b.y; out[3 * t + 2] = b.z;
+    } else if (mask == nullptr || mask[t / N]) {
+        bias[t] = make_float4(in[3 * t], in[3 * t + 1], in[3 * t + 2], 0.f);
+    }
+}
+
+extern "C" int qs_get_gyro_bias(QsHandle* h, float* bias_dev, void* stream) {
+    if (!h || !bias_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
+    QS_CUDA(cudaSetDevice(h->device));
+    k_gyro_bias<<<blocks_for(h->A), 256, 0, (cudaStream_t)stream>>>(h->gyro_bias, h->A, h->cfg.num_agents, nullptr, bias_dev, nullptr);
+    QS_CUDA(cudaGetLastError());
+    h->launches += 1;
+    note_async(h, (cudaStream_t)stream, false);
+    return QS_OK;
+}
+
+extern "C" int qs_set_gyro_bias(QsHandle* h, const uint8_t* env_mask_dev, const float* bias_dev, void* stream) {
+    if (!h || !bias_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->gyro_bias == nullptr) return fail(QS_ERR_INVALID_ARG, "the gyro bias model is off (qs_set_sensor_noise, gyro_norm_std)");
+    QS_CUDA(cudaSetDevice(h->device));
+    k_gyro_bias<<<blocks_for(h->A), 256, 0, (cudaStream_t)stream>>>(h->gyro_bias, h->A, h->cfg.num_agents, env_mask_dev, nullptr, bias_dev);
     QS_CUDA(cudaGetLastError());
     h->launches += 1;
     note_async(h, (cudaStream_t)stream, false);

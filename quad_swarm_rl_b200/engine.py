@@ -15,6 +15,38 @@ DEFAULT_REW_COEFF = dict(pos=1., effort=0.05, action_change=0., crash=1., orient
                          spin=0.1, vel=0., quadcol_bin=5., quadcol_bin_smooth_max=4., quadcol_bin_obst=5.)  # quadrotor_multi.py:91-94
 
 
+# SensorNoise.__init__ keywords and their defaults, sensor_noise.py:69-76
+SENSOR_NOISE_DEFAULTS = dict(pos_norm_std=0.005, pos_unif_range=0., vel_norm_std=0.01, vel_unif_range=0., quat_norm_std=0.,
+                             quat_unif_range=0., gyro_norm_std=0., gyro_noise_density=0.000175, gyro_random_walk=0.0105,
+                             gyro_bias_correlation_time=1000., bypass=False, acc_static_noise_std=0.002,
+                             acc_dynamic_noise_ratio=0.005, use_numba=False)
+# the parameters that reach an observation (the accelerometer is never observed): the fields of QsSensorNoise
+SENSOR_NOISE_FIELDS = tuple(k for k, _ in L.QsSensorNoise._fields_)
+
+
+def resolve_sense_noise(sense_noise):
+    """The `sense_noise` keyword of QuadrotorEnvMulti (quadrotor_single.py:236-247) -> None (no noise), 'default' (the set
+    compiled into the kernels) or a dict of the SENSOR_NOISE_FIELDS (the custom model, qs_set_sensor_noise).  A dict takes
+    the keywords of SensorNoise(**sense_noise): an unknown key raises TypeError like that call; bypass=True is None; a dict
+    whose observed parameters equal the defaults, without the gyro bias model, is 'default'."""
+    if sense_noise is None or (isinstance(sense_noise, str) and sense_noise == 'default'):
+        return sense_noise
+    if not isinstance(sense_noise, dict):
+        raise ValueError("ERROR: QuadEnv: sense_noise parameter is of unknown type: " + str(sense_noise))
+    for k in sense_noise:
+        if k not in SENSOR_NOISE_DEFAULTS:
+            raise TypeError(f"SensorNoise.__init__() got an unexpected keyword argument '{k}'")
+    p = dict(SENSOR_NOISE_DEFAULTS, **sense_noise)
+    if p['bypass']:
+        return None
+    model = {k: float(p[k]) for k in SENSOR_NOISE_FIELDS}
+    defaults = ('pos_norm_std', 'pos_unif_range', 'vel_norm_std', 'vel_unif_range', 'quat_norm_std', 'quat_unif_range',
+                'gyro_noise_density')
+    if model['gyro_norm_std'] == 0. and all(model[k] == SENSOR_NOISE_DEFAULTS[k] for k in defaults):
+        return 'default'
+    return model
+
+
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
@@ -41,7 +73,8 @@ class QuadSwarmEngine:
         cfg.use_obstacles = int(bool(use_obstacles))
         cfg.num_obstacles = self.num_obstacles
         cfg.use_downwash = int(bool(use_downwash))
-        cfg.sense_noise = 0 if sense_noise is None else 1
+        self.sense_noise = resolve_sense_noise(sense_noise)
+        cfg.sense_noise = 0 if self.sense_noise is None else 1
         cfg.obst_size = float(obst_size)
         cfg.room_dims = (C.c_float * 3)(*[float(x) for x in room_dims])
         cfg.ep_time = float(ep_time)
@@ -62,6 +95,10 @@ class QuadSwarmEngine:
         h = C.c_void_p()
         L.check(self.lib.qs_create(C.byref(cfg), int(device), C.byref(h)))
         self.h = h
+        # stateful gyro model on: get_state() / set_state() carry the per-drone gyro bias
+        self.gyro_model = isinstance(self.sense_noise, dict) and self.sense_noise['gyro_norm_std'] != 0.
+        if isinstance(self.sense_noise, dict):
+            L.check(self.lib.qs_set_sensor_noise(h, C.byref(L.QsSensorNoise(**self.sense_noise))))
         self.D = self.lib.qs_obs_dim(h)
         self.M = self.lib.qs_num_obstacles(h)
         self.ep_len = self.lib.qs_ep_len(h)
@@ -196,7 +233,10 @@ class QuadSwarmEngine:
         ei = torch.empty((self.E, L.QS_STATE_ENV_I32), dtype=torch.int32, device=dev)
         ob = torch.empty((self.E, max(self.M, 1), 2), dtype=torch.float32, device=dev)
         L.check(self.lib.qs_get_state(self.h, _ptr(af), _ptr(au), _ptr(ei), _ptr(ob), self._stream()))
-        return dict(agent_f32=af, agent_u32=au, env_i32=ei, obst_xy=ob[:, :self.M])
+        st = dict(agent_f32=af, agent_u32=au, env_i32=ei, obst_xy=ob[:, :self.M])
+        if self.gyro_model:
+            st['gyro_bias'] = self.get_gyro_bias()
+        return st
 
     def set_state(self, state, env_mask=None):
         af = state['agent_f32'].to(self.device, torch.float32).contiguous()
@@ -206,6 +246,19 @@ class QuadSwarmEngine:
         ob = ob.to(self.device, torch.float32).contiguous() if (ob is not None and self.M > 0) else None
         m = self._dev_mask(env_mask)
         L.check(self.lib.qs_set_state(self.h, _ptr(m), _ptr(af), _ptr(au), _ptr(ei), _ptr(ob), self._stream()))
+        if self.gyro_model and state.get('gyro_bias') is not None:
+            self.set_gyro_bias(state['gyro_bias'], env_mask=env_mask)
+
+    def get_gyro_bias(self):
+        """Gyro bias of every drone [E,N,3] (zeros unless the stateful gyro model is on)."""
+        b = torch.empty((self.E, self.N, 3), dtype=torch.float32, device=self.device)
+        L.check(self.lib.qs_get_gyro_bias(self.h, _ptr(b), self._stream()))
+        return b
+
+    def set_gyro_bias(self, bias, env_mask=None):
+        b = self._dev_f32(bias, (self.E, self.N, 3))
+        m = self._dev_mask(env_mask)
+        L.check(self.lib.qs_set_gyro_bias(self.h, _ptr(m), _ptr(b), self._stream()))
 
     def episode_stats(self):
         dev = self.device

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .engine import QuadSwarmEngine
+from .engine import QuadSwarmEngine, resolve_sense_noise
 from .scenarios import create_scenario, obstacle_map_given_density
 from .spaces import make_observation_space, make_action_space
 
@@ -94,8 +94,7 @@ class _EnvBase:
             raise NotImplementedError("init_random_state=True is not supported")
         if quads_render:
             raise NotImplementedError("rendering is out of scope")
-        if sense_noise not in ('default', None):
-            raise ValueError("ERROR: QuadEnv: sense_noise parameter is of unknown type: " + str(sense_noise))
+        resolve_sense_noise(sense_noise)                     # 'default', None or a dict of SensorNoise parameters
         self.num_envs = int(num_envs)
         self.num_agents_per_env = int(num_agents)
         self.is_multiagent = True                           # quadrotor_multi.py:54
