@@ -283,6 +283,18 @@ int qs_set_sensor_noise(QsHandle* h, const QsSensorNoise* noise_host);
 int qs_get_gyro_bias(QsHandle* h, float* bias_dev, void* stream);
 int qs_set_gyro_bias(QsHandle* h, const uint8_t* env_mask_dev, const float* bias_dev, void* stream);
 
+/* Random initial states — replaces QuadrotorSingle(init_random_state=True) (quadrotor_single.py:405-423, 3-D): every spawn of
+ * every drone, explicit reset or auto-reset, starts from QuadrotorDynamics.random_state (quadrotor_dynamics.py:193-206)
+ * instead of a level attitude facing the origin at rest:
+ *   vel = m / (|d| + 1e-6) d, d ~ U(-vel_max, vel_max)^3, m ~ U(0, vel_max); omega likewise with omega_max;
+ *   R = rand_uniform_rot3d() (quad_utils.py:94-104), uniform over SO(3), upside down included.
+ * The position is the usual spawn jitter (z >= 0.75); the neighbour block of a reset observation still sees the stale
+ * velocities (QuadrotorEnvMulti.reset does not refresh self.vel).  The reference's values are vel_max = 1 m/s and
+ * omega_max = 2 pi rad/s (QuadrotorSingle.max_init_vel / max_init_omega, quadrotor_single.py:181-182); both must be finite
+ * and >= 0.  enable = 0 restores the default.  Call after qs_create and before the first qs_reset / qs_step; later calls fail
+ * with QS_ERR_INVALID_ARG (the reference fixes the option in its constructor).  Works in every step shape. */
+int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega_max);
+
 /* flag bits in agent_u32[.,0] */
 #define QS_FLAG_ON_FLOOR (1u << 0)
 #define QS_FLAG_CRASHED_FLOOR (1u << 1)

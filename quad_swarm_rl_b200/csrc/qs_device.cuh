@@ -143,6 +143,8 @@ struct StepParams {
     NoiseModel nz;                      // custom sensor-noise model (NZ instantiations)
     float4* gyro_bias;                  // [A] xyz: gyro bias of the stateful gyro model (qs_set_sensor_noise), or null: model off
                                         // (not in DevState: the scenario functions take that by value)
+    int init_random;                    // qs_set_init_random_state: every spawn gets a random vel / omega / R (random_init_state)
+    float init_vel_max, init_omega_max;
 };
 
 struct Agent {
@@ -994,6 +996,51 @@ __device__ __forceinline__ void apply_reset(Agent& s, const ResetPose& r) {
     for (int m = 0; m < 4; ++m) { s.rd[m] = 0.f; s.cd[m] = 0.f; s.ring[m] = 0.f; }
     s.flags = QS_FLAG_NO_COL_AGENT | QS_FLAG_NO_COL_OBST;
     s.prev_col = 0u;
+}
+
+// normalize(), quad_utils.py:80-86: a vector shorter than 1e-5 is returned unchanged
+__device__ __forceinline__ V3 normalize_ref(V3 v) {
+    const float n = sqrtf(v.x * v.x + v.y * v.y + v.z * v.z);
+    if (n < 0.00001f) return v;
+    v.x /= n; v.y /= n; v.z /= n;
+    return v;
+}
+
+// The initial state of a spawn with init_random_state (quadrotor_single.py:405-423): QuadrotorDynamics.random_state
+// (quadrotor_dynamics.py:193-206).  Velocity and body rate: a direction from a uniform cube, scaled to a uniform magnitude,
+// x = mag / (|d| + EPS) d with EPS = 1e-6 (:13); attitude: rand_uniform_rot3d (quad_utils.py:94-104), R = [fwd | left | up].
+// random_state's position draw is discarded by _reset and not drawn here.  The fwd re-draw loop is capped at
+// INIT_ROT_MAX_TRIES (DESIGN, deviations).  Keyed by the episode, like the spawn jitter: applied after apply_reset.
+struct InitState { float vel[3], om[3], R[9]; };
+__device__ __noinline__ InitState random_init_state(RngKey key, int i, float vel_max, float omega_max) {
+    InitState o;
+    const float4 u0 = rng_uniform4(key, SITE_INIT_U, i, 0, 0), u1 = rng_uniform4(key, SITE_INIT_U, i, 0, 1);
+    {
+        const float lo = -vel_max, w = vel_max - lo;
+        const float dx = lo + w * u0.x, dy = lo + w * u0.y, dz = lo + w * u0.z;
+        const float f = (vel_max * u0.w) / (sqrtf(dx * dx + dy * dy + dz * dz) + 1e-6f);
+        o.vel[0] = f * dx; o.vel[1] = f * dy; o.vel[2] = f * dz;
+    }
+    {
+        const float lo = -omega_max, w = omega_max - lo;
+        const float dx = lo + w * u1.x, dy = lo + w * u1.y, dz = lo + w * u1.z;
+        const float f = (omega_max * u1.w) / (sqrtf(dx * dx + dy * dy + dz * dz) + 1e-6f);
+        o.om[0] = f * dx; o.om[1] = f * dy; o.om[2] = f * dz;
+    }
+    const float4 nu = rng_normal4(key, SITE_INIT_N, i, 0, 0);
+    V3 up = normalize_ref(V3{nu.x, nu.y, nu.z}), fwd;
+#pragma unroll 1
+    for (int t = 0; t < INIT_ROT_MAX_TRIES; ++t) {
+        const float4 nf = rng_normal4(key, SITE_INIT_N, i, 0, t + 1);
+        fwd = normalize_ref(V3{nf.x, nf.y, nf.z});
+        if (!(fwd.x * up.x + fwd.y * up.y + fwd.z * up.z > 0.95f)) break;
+    }
+    const V3 left = normalize_ref(V3{up.y * fwd.z - up.z * fwd.y, up.z * fwd.x - up.x * fwd.z, up.x * fwd.y - up.y * fwd.x});
+    up = V3{fwd.y * left.z - fwd.z * left.y, fwd.z * left.x - fwd.x * left.z, fwd.x * left.y - fwd.y * left.x};
+    o.R[0] = fwd.x; o.R[1] = left.x; o.R[2] = up.x;
+    o.R[3] = fwd.y; o.R[4] = left.y; o.R[5] = up.y;
+    o.R[6] = fwd.z; o.R[7] = left.z; o.R[8] = up.z;
+    return o;
 }
 
 }  // namespace qs

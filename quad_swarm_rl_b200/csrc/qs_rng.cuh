@@ -45,9 +45,14 @@ enum Site : uint32_t {
     SITE_NOISE_N = 18,      // (i,j) normals v0..2 pos, v4..6 vel, v8..10 gyro, v12..14 rotation angle   sensor_noise.py:241-256
     SITE_NOISE_U = 19,      // (i,j) uniforms v0..2 pos, v4..6 vel, v8..10 rotation angle
     SITE_GYRO_BIAS = 20,    // (i,j) normals v0..2 bias innovation, v4..6 random walk                    sensor_noise.py:221-231
+    // Random initial state of a spawn (qs_set_init_random_state; QuadrotorDynamics.random_state, quadrotor_dynamics.py:193-206),
+    // episode-keyed like SITE_SPAWN_U.  Full-precision draws; CPU twin: oracle/init_state_oracle.py.
+    SITE_INIT_U = 21,       // (i)   uniforms v0..2 vel direction, v3 vel magnitude, v4..6 omega direction, v7 omega magnitude
+    SITE_INIT_N = 22,       // (i)   normals v0..2 up, v[4(t+1)..4(t+1)+2] fwd of try t        rand_uniform_rot3d, quad_utils.py:94-104
 };
 
 constexpr int RESET_YAW_MAX_TRIES = 64;
+constexpr int INIT_ROT_MAX_TRIES = 16;      // fwd re-draws of rand_uniform_rot3d (reference: unbounded; p(re-draw) ~ 2.5 %)
 
 struct RngKey {
     uint32_t k0, k1;      // seed
@@ -58,7 +63,8 @@ struct RngKey {
 // Draws that define an EPISODE (pillar / spawn / goal generation, formation picks, spawn jitter, reset yaw) are keyed by the
 // env's episode number, not by its step counter: counter word 1 = EPISODE_KEY_BIT | episode number.  An episode is then a
 // function of (seed, env id, episode number) only, whenever and wherever it is generated — inside the reset path of the
-// step kernel, or ahead of time by qs_pregen_kernel.  Sites: SITE_SCENARIO_U streams 0 / 1, SITE_SPAWN_U, SITE_RESET_YAW_U.
+// step kernel, or ahead of time by qs_pregen_kernel.  Sites: SITE_SCENARIO_U streams 0 / 1, SITE_SPAWN_U, SITE_RESET_YAW_U,
+// SITE_INIT_U, SITE_INIT_N.
 constexpr uint32_t EPISODE_KEY_BIT = 0x80000000u;
 
 constexpr uint32_t PHILOX_M0 = 0xD2511F53u, PHILOX_M1 = 0xCD9E8D57u, PHILOX_W0 = 0x9E3779B9u, PHILOX_W1 = 0xBB67AE85u;

@@ -363,11 +363,12 @@ __device__ __forceinline__ EpisodeLane generate_episode(const StepParams& p, con
 
 // Start the next episode of one env and respawn its drones (QuadrotorEnvMulti.reset, quadrotor_multi.py:339-411).
 // Called by ALL lanes of a warp (the branch around it is warp-uniform); `do_reset` is per env.  Sets nvel to the velocity
-// the neighbour block must see.
+// the neighbour block must see.  init_random: the spawns get random initial states (p.init_random; a compile-time constant
+// in the reset kernel).
 template <int NP, bool SCN>
 __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key, Agent& s, long long a, int env, int i,
                                           bool do_reset, bool valid, int tick_before_reset, float2* s_obst_env,
-                                          float nvel[3], int& scn_next, float& approach, float& obst_r) {
+                                          float nvel[3], int& scn_next, float& approach, float& obst_r, bool init_random) {
     const DevState& st = p.st;
     if (do_reset && valid) {
         // stale velocity (Appendix D-6): the multi-env's self.vel is only refreshed by step()
@@ -425,6 +426,13 @@ __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key
         }
         if (i == 0) st.epi[env] = make_int2(g, ep.y);
         apply_reset(s, rp);
+        if (init_random) {          // a handle-wide setting; episode-keyed, so a pre-generated record needs no extra field
+            const InitState r = random_init_state(episode_key(p, env, g), i, p.init_vel_max, p.init_omega_max);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { s.vel[k] = r.vel[k]; s.om[k] = r.om[k]; }
+#pragma unroll
+            for (int k = 0; k < 9; ++k) s.R[k] = r.R[k];
+        }
         st.slots[SL_DIST_SUMS * st.a_pad + a] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     if (p.use_obst) {
@@ -1211,7 +1219,8 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
                 o[QS_STAT_EPISODES_DONE] = ctr.episode_idx + 1;
                 o[QS_STAT_SCENARIO] = (dev_scn || env_metric) ? QS_LD(st.scn_i + env).x : p.scenario;
             }
-            reset_env<NP, SCN>(p, key, s, a, env, i, do_reset, valid, ctr.tick, SPLIT ? nullptr : s_obst_env, nvel, scn_next, approach, obst_r);
+            reset_env<NP, SCN>(p, key, s, a, env, i, do_reset, valid, ctr.tick, SPLIT ? nullptr : s_obst_env, nvel, scn_next, approach, obst_r,
+                               p.init_random != 0);
             if (DYN) {
                 // resample_dynamics inside _reset (quadrotor_single.py:387-390): constants uploaded with at_next_reset are
                 // latched now; update_dynamics builds a fresh QuadrotorDynamics, so OU state and SVD counter restart
@@ -1352,7 +1361,8 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
 }
 
 // Explicit reset of the masked envs: QuadrotorEnvMulti.reset, quadrotor_multi.py:339-411.  NZ: custom sensor-noise model.
-template <int NP, bool NZ = false>
+// RND: random initial states (qs_set_init_random_state).
+template <int NP, bool NZ = false, bool RND = false>
 __global__ void __launch_bounds__(128) qs_reset_kernel(const __grid_constant__ StepParams p) {
     extern __shared__ __align__(128) float2 s_obst[];
     const DevState& st = p.st;
@@ -1391,7 +1401,7 @@ __global__ void __launch_bounds__(128) qs_reset_kernel(const __grid_constant__ S
     int scn_next = SCN_NEVER;
     float approach = p.approach_metric;
     float obst_r = p.obst_radius;
-    reset_env<NP, true>(p, key, s, a, env, i, env_ok, valid, ctr.tick, s_obst_env, nvel, scn_next, approach, obst_r);
+    reset_env<NP, true>(p, key, s, a, env, i, env_ok, valid, ctr.tick, s_obst_env, nvel, scn_next, approach, obst_r, RND);
     if (st.dyn != nullptr) {          // pending physical constants are latched by explicit resets too
         const int pend = env_ok ? QS_LD(st.dyn_pending + env) : 0;
         if (pend != 0) {

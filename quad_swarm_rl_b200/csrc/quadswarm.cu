@@ -55,7 +55,9 @@ struct QsHandle {
     bool nz_on;           // qs_set_sensor_noise: the custom sensor-noise model (NZ kernels)
     NoiseModel nz;
     float4* gyro_bias;    // [A], allocated when the gyro bias model is on
-    bool started;         // a reset or step has been enqueued: the noise model is fixed from here on
+    bool started;         // a reset or step has been enqueued: the noise model and the initial-state mode are fixed from here on
+    int init_random;      // qs_set_init_random_state
+    float init_vel_max, init_omega_max;
     cudaStream_t last_stream;   // stream of the most recent asynchronous call of this handle
     bool async_pending;
     // staging for the *_host entry points (pinned host + device mirrors)
@@ -129,6 +131,7 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.scenario = c.scenario; p.grid_l = c.obst_grid[0]; p.grid_w = c.obst_grid[1];
     p.nz = h->nz;
     p.gyro_bias = h->gyro_bias;
+    p.init_random = h->init_random; p.init_vel_max = h->init_vel_max; p.init_omega_max = h->init_omega_max;
 }
 
 // Observation write-out mode of a step launch (qs_step.cuh, emit_observation_tile): the bulk-copy engine needs a 16-byte
@@ -560,8 +563,12 @@ static int launch_reset(QsHandle* h, const StepParams& p, cudaStream_t s) {
     const int grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
     const size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
     int rc = dispatch_np(h->NP, [&](auto np) {
-        if (h->nz_on) qs_reset_kernel<decltype(np)::value, true><<<grid, kBlock, smem, s>>>(p);
-        else qs_reset_kernel<decltype(np)::value><<<grid, kBlock, smem, s>>>(p);
+        constexpr int NPv = decltype(np)::value;
+        if (h->init_random) {
+            if (h->nz_on) qs_reset_kernel<NPv, true, true><<<grid, kBlock, smem, s>>>(p);
+            else qs_reset_kernel<NPv, false, true><<<grid, kBlock, smem, s>>>(p);
+        } else if (h->nz_on) qs_reset_kernel<NPv, true><<<grid, kBlock, smem, s>>>(p);
+        else qs_reset_kernel<NPv><<<grid, kBlock, smem, s>>>(p);
         return QS_OK;
     });
     if (rc != QS_OK) return rc;
@@ -948,6 +955,17 @@ extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const f
     QS_CUDA(cudaGetLastError());
     h->launches += 1;
     note_async(h, (cudaStream_t)stream, false);
+    return QS_OK;
+}
+
+extern "C" int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega_max) {
+    if (!h) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->started) return fail(QS_ERR_INVALID_ARG, "the initial-state mode can only be set before the first reset or step");
+    if (!(vel_max >= 0.f) || !std::isfinite(vel_max) || !(omega_max >= 0.f) || !std::isfinite(omega_max))
+        return fail(QS_ERR_INVALID_ARG, "vel_max and omega_max must be finite and >= 0");
+    h->init_random = enable ? 1 : 0;
+    h->init_vel_max = vel_max;
+    h->init_omega_max = omega_max;
     return QS_OK;
 }
 

@@ -5,6 +5,7 @@ and stream plumbing: every tensor handed to the C ABI is a plain device pointer.
 object protocol (QuadrotorEnvMulti.reset()/step()) lives in env.py on top of this class.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -57,7 +58,7 @@ class QuadSwarmEngine:
                  obst_spawn_area=(8.0, 8.0), use_downwash=False, room_dims=(10., 10., 10.), ep_time=15.0,
                  collision_hitbox_radius=2.0, collision_falloff_radius=4.0, sense_noise='default',
                  approch_goal_metric=0.5, rew_coeff=None, seed=0, device=0, env_id_offset=0,
-                 device_scenario=None, quad_arm=0.0):
+                 device_scenario=None, quad_arm=0.0, init_random_state=False, init_vel_max=1.0, init_omega_max=2 * math.pi):
         if not torch.cuda.is_available():
             raise RuntimeError("QuadSwarmEngine needs a CUDA device (the env step has no CPU path)")
         self.lib = L.load()
@@ -99,6 +100,11 @@ class QuadSwarmEngine:
         self.gyro_model = isinstance(self.sense_noise, dict) and self.sense_noise['gyro_norm_std'] != 0.
         if isinstance(self.sense_noise, dict):
             L.check(self.lib.qs_set_sensor_noise(h, C.byref(L.QsSensorNoise(**self.sense_noise))))
+        # QuadrotorSingle(init_random_state=True): every spawn starts from a random velocity, body rate and attitude
+        # (max_init_vel / max_init_omega, quadrotor_single.py:181-182)
+        self.init_random_state = bool(init_random_state)
+        if self.init_random_state:
+            L.check(self.lib.qs_set_init_random_state(h, 1, float(init_vel_max), float(init_omega_max)))
         self.D = self.lib.qs_obs_dim(h)
         self.M = self.lib.qs_num_obstacles(h)
         self.ep_len = self.lib.qs_ep_len(h)

@@ -90,8 +90,6 @@ class _EnvBase:
             raise AttributeError(f"module 'quadrotor_randomization' has no attribute {dynamics_params!r}")     # getattr(quad_rand, name)
         if not (raw_control and raw_control_zero_middle):
             raise NotImplementedError("only RawControl with zero_action_middle is supported")
-        if init_random_state:
-            raise NotImplementedError("init_random_state=True is not supported")
         if quads_render:
             raise NotImplementedError("rendering is out of scope")
         resolve_sense_noise(sense_noise)                     # 'default', None or a dict of SensorNoise parameters
@@ -161,6 +159,7 @@ class _EnvBase:
             ep_time=ep_time, collision_hitbox_radius=collision_hitbox_radius,
             collision_falloff_radius=collision_falloff_radius, sense_noise=sense_noise, rew_coeff=rew_coeff,
             seed=seed, device=device, env_id_offset=env_id_offset, device_scenario=device_scenario, quad_arm=quad_arm,
+            init_random_state=init_random_state,
             # scenario.approch_goal_metric (o_base.py:16: 1.0 for the goal-sharing obstacle scenarios, else 0.5); with the
             # host-side `mix` over obstacle scenarios the value of o_random is used for every episode
             approch_goal_metric=1.0 if quads_mode in ('o_static_same_goal', 'o_dynamic_same_goal', 'o_swap_goals',
@@ -478,7 +477,7 @@ class QuadrotorEnvMultiBatched(_EnvBase):
                  obst_spawn_area=(8.0, 8.0), use_downwash=False, quads_mode='static_same_goal',
                  room_dims=(10., 10., 10.), sense_noise='default', device=0, seed=None, env_id_offset=0,
                  device_scenarios=True, dynamics_params='Crazyflie', dynamics_randomize_every=None, dynamics_change=None,
-                 dyn_sampler_1=None):
+                 dyn_sampler_1=None, init_random_state=False):
         # device-side generators (no host work per episode or per tick): o_random with obstacles, the goal-formation
         # family and mix without; every other mode uses host tables
         dev_scn = None
@@ -489,8 +488,8 @@ class QuadrotorEnvMultiBatched(_EnvBase):
         super().__init__(num_envs, num_agents, ep_time, rew_coeff, obs_repr, neighbor_visible_num, neighbor_obs_type,
                          collision_hitbox_radius, collision_falloff_radius, use_obstacles, obst_density, obst_size,
                          obst_spawn_area, use_downwash, True, quads_mode, room_dims, False, ['topdown'], False,
-                         dynamics_params, True, True, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise, False,
-                         device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn)
+                         dynamics_params, True, True, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise,
+                         init_random_state, device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn)
         self.num_agents = num_envs * num_agents
         self._truncated = torch.zeros(self.num_agents, dtype=torch.bool, device=self.engine.device)
 
