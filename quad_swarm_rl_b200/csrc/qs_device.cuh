@@ -78,7 +78,7 @@ struct DevState {
     float2* next_obst;      // [E][M]
     int32_t* stats_env;     // [E][QS_NUM_ENV_STATS]  latched at episode end
     float4* stats_agent;    // [A]                     latched at episode end
-    int* ready;             // [E + 1] per step-kernel block: 1 = the block's env state is complete in L2 (pdl_mode 3);
+    int* ready;             // [E + 1] per step-kernel block: 1 = the block's env state is complete in L2 (per-block hand-over);
                             //         ready[E] counts hand-over waits that timed out
     int2* epi;              // [E] x = number of the episode the env is running (every reset, explicit or automatic, starts the
                             //     next one; keys the episode-generation draws), y = episode number the next-episode RECORD
@@ -133,13 +133,10 @@ struct StepParams {
     int obst_counts[QS_MAX_OBST_CHOICES];
     float obst_radii[QS_MAX_OBST_CHOICES];
     int chained;                        // 1: the stream predecessor of this launch is a step grid of the same handle (qs_set_chained):
+                                        //    actions are prefetched before the dependency wait; hand-over kernels skip the grid-wide wait
     int courier;            // per-block hand-over with a courier warp (last warp of the block, no envs): early release of the state
     int wrap_chain;         // courier launch inside qs_wrap_step: block-chained with the wrapper kernel (see qs_wrap_kernel)
-    int poll_mode;          // how the courier polls for its turn (counter_wait, QS_POLL)
-                                        //    actions are prefetched before the dependency wait; hand-over kernels skip the grid-wide wait
     int scenario, grid_l, grid_w;       // QS_SCENARIO_*, pillar grid cells along x / y
-    int pdl_mode;                       // 0 off, 1 trigger dependents at kernel start, 2 trigger before the final stores,
-                                        // 3 per-block hand-over: no grid-wide wait at all (see qs_step_kernel)
     NoiseModel nz;                      // custom sensor-noise model (NZ instantiations)
     float4* gyro_bias;                  // [A] xyz: gyro bias of the stateful gyro model (qs_set_sensor_noise), or null: model off
                                         // (not in DevState: the scenario functions take that by value)

@@ -449,9 +449,7 @@ __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key
 
 // 8 worker warps + the courier: c3 / c5 (1024 physics warps) keep the courier on 132 SMs.  One such CTA per SM (~130-170
 // registers); two per SM (<= 112 registers) spill, and on H100 were slower on c5, c2 and the wrapped step.
-#ifndef QS_LB
 #define QS_LB 288
-#endif
 // named barriers of the split kernel (physics warp <-> observer warp, 64 threads).  Both warps use bar.sync: the
 // observer reaches barrier 1 first, the physics warp reaches barrier 2 first and has only its stores left to do.
 // Out of line on purpose: both warps then execute the SAME bar.sync instruction (what compute-sanitizer's synccheck
@@ -490,7 +488,7 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, int parity) {
 // round trip per counter on the critical path of every warp with a discrete event.
 __device__ __forceinline__ void cnt_add(int32_t* c, int k, int v) { if (v != 0) atomicAdd(c + k, v); }
 
-// ---- per-block hand-over between consecutive step grids (pdl_mode 3) ----
+// ---- per-block hand-over between consecutive step grids (HO kernels) ----
 // Envs are independent, so block b of step t+1 only needs block b of step t.  Every step launch carries the programmatic
 // stream-serialization attribute; instead of griddepcontrol.wait (a grid-wide barrier: every step then costs the launch
 // latency plus the SLOWEST warp of the grid) a block waits for its own predecessor's `ready` word, takes it, and only
@@ -534,23 +532,12 @@ __device__ __forceinline__ void handover_release(int* ready) {
 // At rest T = S = D and Tw = Dw = Rw; an unchained launch needs no special case.
 enum { HW_READY = 0, HW_T = 1, HW_S = 2, HW_D = 3, HW_TW = 4, HW_DW = 5, HW_RW = 6, HW_ROWS = 7 };     // rows of DevState::ready, [E + 1] each
 __device__ __forceinline__ int* hw_word(const DevState& st, int E, int row) { return st.ready + (long long)row * (E + 1) + blockIdx.x; }
-// mode (tuning, QS_POLL): bits 0-7 = nanoseconds to sleep between two polls, bit 8 = poll with relaxed loads and fence once at
-// the end (an ld.acquire is LDG.STRONG + CCTL.IVALL: every poll then invalidates the SM's L1, also for the co-resident CTA)
-__device__ __forceinline__ void counter_wait(const int* c, int want, int* timeouts, int* err_flag, int mode = 40) {
+__device__ __forceinline__ void counter_wait(const int* c, int want, int* timeouts, int* err_flag) {
     int v = 0, spins = 0;
-    const unsigned ns = (unsigned)(mode & 0xff);
-    if (mode & 0x100) {
-        do {
-            asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(c) : "memory");
-            if (v - want < 0 && ns) __nanosleep(ns);
-        } while (v - want < 0 && ++spins < (1 << 24));
-        asm volatile("fence.acq_rel.gpu;" ::: "memory");
-    } else {
-        do {
-            asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(c) : "memory");
-            if (v - want < 0 && ns) __nanosleep(ns);
-        } while (v - want < 0 && ++spins < (1 << 24));    // ~1 s: a lost hand-over must not hang the GPU
-    }
+    do {
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(c) : "memory");
+        if (v - want < 0) __nanosleep(40);
+    } while (v - want < 0 && ++spins < (1 << 24));    // ~1 s: a lost hand-over must not hang the GPU
     if (v - want < 0) {
         atomicAdd(timeouts, 1);
         if (err_flag != nullptr) *reinterpret_cast<volatile int*>(err_flag) = 1;
@@ -627,7 +614,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         }
         named_arrive(5, nthr);                                        // ... is taken before any thread of the block lets the next grid launch
         asm volatile("griddepcontrol.launch_dependents;");
-        if (lane == 0) counter_wait(hw_word(st, p.E, HW_S), k, tmo, st.err_flag, p.poll_mode);
+        if (lane == 0) counter_wait(hw_word(st, p.E, HW_S), k, tmo, st.err_flag);
         named_arrive(1, nthr);                                        // the workers start loading the state
         if (lane == 0) {
             // the predecessor's observation rows are out (in a wrapped chain the wrapper kernel has waited for that)
@@ -668,8 +655,8 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
 
     // Programmatic dependent launch: wait here for the PREVIOUS step's grid to complete (and flush) before touching any
     // state; the trigger that lets the NEXT step's grid start launching is issued just before this grid's final stores
-    // (mode 2, default: hides part of the launch latency of each step; triggering at kernel start, mode 1, is SLOWER
-    // because the early grid competes for issue slots while it spins).  Without the launch attribute both are no-ops.
+    // (hides part of the launch latency of each step; triggering at kernel start is SLOWER because the early grid competes
+    // for issue slots while it spins).  Without the launch attribute both are no-ops.
     if (HO) {
         // not chained: the stream predecessor may be a foreign kernel (it never triggers early, so this grid starts when
         // it has completed; the wait makes its writes formally visible).  Chained step grids (qs_set_chained) skip it.
@@ -684,9 +671,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             asm volatile("griddepcontrol.launch_dependents;");
         }
     } else {
-        if (p.pdl_mode == 1) asm volatile("griddepcontrol.launch_dependents;");
         asm volatile("griddepcontrol.wait;" ::: "memory");
-        if (p.pdl_mode == 4) asm volatile("griddepcontrol.launch_dependents;");      // trigger once the predecessor is done
     }
 
     QS_TL(1);
@@ -833,7 +818,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             ctr.step_count += 1;
             bar_sync(3);                                              // hand-off arrays and tile are free again
         }
-        if (p.pdl_mode == 2) asm volatile("griddepcontrol.launch_dependents;");
+        if (!HO) asm volatile("griddepcontrol.launch_dependents;");
         if (HO) bar_sync(4);                                          // the physics warp publishes the block's state
         return;
     }
@@ -889,11 +874,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         s.ou[1] += OU_THETA * (0.f - s.ou[1]) + ou_sigma * ou_z.y;
         s.ou[2] += OU_THETA * (0.f - s.ou[2]) + ou_sigma * ou_z.z;
         s.ou[3] += OU_THETA * (0.f - s.ou[3]) + ou_sigma * ou_z.w;
-#ifdef QS_UNROLL_SUB
-#pragma unroll
-#else
 #pragma unroll 1
-#endif
         for (int sub = 0; sub < SIM_STEPS; ++sub) {
             ctr.svd_count += 1;
             const bool do_svd = ctr.svd_count >= SVD_PERIOD;
@@ -934,11 +915,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         if (NP > 1) {
             const float max_pen = p.rew[QS_REW_QUADCOL_BIN_SMOOTH_MAX];
             const float pen_ratio = -max_pen / p.falloff_thr;
-#ifndef QS_PASSA_UNROLL
-#define QS_PASSA_UNROLL 2
-#endif
-            constexpr int kPassAUnroll = QS_PASSA_UNROLL;
-#pragma unroll kPassAUnroll
+#pragma unroll 2
             for (int j = 0; j < p.N; ++j) {
                 const float dx = s.pos[0] - shfl<NP>(s.pos[0], j), dy = s.pos[1] - shfl<NP>(s.pos[1], j),
                             dz = s.pos[2] - shfl<NP>(s.pos[2], j);
@@ -1338,7 +1315,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         ctr.step_count += 1;
     }
 
-    if (p.pdl_mode == 2) asm volatile("griddepcontrol.launch_dependents;");     // late trigger: overlap only the launch latency
+    if (!HO) asm volatile("griddepcontrol.launch_dependents;");                 // late trigger: overlap only the launch latency
     QS_TL(6);
     if (!stored_early || late_goal) {
         if (valid) store_agent(st, a, s, goal_dirty);

@@ -21,15 +21,15 @@ using namespace qs;
 struct QsHandle {
     QsConfig cfg;
     int device;
+    int sms;              // multiprocessors of the device
     int NP;               // lanes per env (next pow2 >= N)
     int K, S, D, M, ep_len;
     long long A, a_pad;
     DevState st;
     float rew[QS_NUM_REW_COEFF];
     int64_t launches;
-    int split_mode;       // -1 auto, 0 single-warp kernel, 1 split kernel (QS_SPLIT, read at qs_create)
-    int pdl_env;          // QS_PDL at the first step launch (-2 = not read yet, -1 = unset)
-    int handover;         // -1 not decided yet, 0 grid-wide wait between step grids, 1 per-block hand-over (launch_step)
+    int split_mode;       // -1 auto, 0 single-warp kernel, 1 split kernel (QS_SPLIT)
+    int handover;         // -1 not decided yet, 0 grid-wide wait between step grids, 1 per-block hand-over (plan_step; QS_PDL)
     int obst_random, n_obst_counts, n_obst_radii;
     int obst_counts[QS_MAX_OBST_CHOICES];
     float obst_radii[QS_MAX_OBST_CHOICES];
@@ -38,14 +38,13 @@ struct QsHandle {
     float* wrap_agg_host; // pinned
     int pregen_every;     // step launches between two launches of the next-episode generator (0 = never), QS_PREGEN overrides
     int since_pregen;
-    unsigned long long capture_id;   // id of the stream capture that saw the last generator launch at its head
     int chained;          // qs_set_chained: consecutive qs_step / qs_rollout launches follow each other directly on the stream
     int last_was_step;    // the last launch this handle enqueued was a step / rollout grid
     int last_was_wrap;    // ... was the wrapper kernel of a wrapped control step launched block-chained (qs_wrap_step)
     int in_wrap_step;     // launch_step is called from qs_wrap_step
     int step_wrap_chain;  // the step grid just launched leaves its blocks to the wrapper kernel (StepParams.wrap_chain)
     int wrap_block;       // worker threads per block of that step grid (the wrapper kernel uses the same env -> block mapping)
-    int bulk_mode;        // QS_OBS_BULK: -1 auto, 0 never use the bulk-copy engine for the observation write-out, 2 linear copies only
+    int bulk_mode;        // QS_OBS_BULK: 0 never use the bulk-copy engine for the observation write-out, else automatic
     int* err_host;        // mapped page-locked word the step kernels set when a hand-over wait timed out (sticky)
     cudaEvent_t ev_sync;  // the *_host entry points (own stream) order themselves after the caller-stream work below
 #ifdef QS_TIMELINE
@@ -159,7 +158,7 @@ static void choose_obs_writeout(const QsHandle* h, StepParams& p, bool dst_is_de
     static_assert(sizeof(CUtensorMap) == sizeof(p.obs_map), "tensor map size");
     if (!p.obs_stage || !dst_is_device_memory || h->bulk_mode == 0) return;
     if (((uintptr_t)p.obs & 15u) != 0) return;
-    if (p.D % 4 == 0 && h->bulk_mode != 2) {
+    if (p.D % 4 == 0) {
         // tensor map of the caller's observation array: [T][A][D] floats, box [1][rows of a warp tile][Dp] — the box is as
         // wide as the padded shared-memory row; the columns >= D (and rows >= A of a ragged last tile) are clipped
         EncodeTiledFn enc = tensor_map_encoder();
@@ -337,17 +336,6 @@ __global__ void k_read_stats(DevState st, int E, int N, int32_t* env_stats, floa
 // ------------------------------------------------------------------------------------------
 // launch helpers
 // ------------------------------------------------------------------------------------------
-static int block_size() {
-    // threads per CTA (multiple of 32, <= 128); QS_BLOCK overrides for tuning experiments
-    static int b = 0;
-    if (b == 0) {
-        const char* e = getenv("QS_BLOCK");
-        b = e ? atoi(e) : 64;
-        if (b < 32 || b > QS_LB || (b % 32) != 0) b = 64;
-    }
-    return b;
-}
-
 template <typename F>
 static int dispatch_np(int NP, F&& f) {
     switch (NP) {
@@ -361,176 +349,143 @@ static int dispatch_np(int NP, F&& f) {
     return fail(QS_ERR_UNSUPPORTED, "num_agents > 32 is not supported by this build");
 }
 
+using KernelFn = void (*)(StepParams);
+
+template <int NP, bool SPLIT, bool HO, bool DYN, bool NZ>
+static KernelFn step_kernel_scn(bool scn) {
+    return scn ? (KernelFn)qs_step_kernel<NP, SPLIT, true, HO, DYN, NZ> : (KernelFn)qs_step_kernel<NP, SPLIT, false, HO, DYN, NZ>;
+}
+
+// The step-kernel instantiation of a launch.  DYN and NZ exist only in the single-warp shape with the grid-wide wait, so
+// `split` and `ho` do not apply to them.
+template <int NP>
+static KernelFn step_kernel(bool split, bool scn, bool ho, bool dyn, bool nz) {
+    if (nz) return dyn ? step_kernel_scn<NP, false, false, true, true>(scn) : step_kernel_scn<NP, false, false, false, true>(scn);
+    if (dyn) return step_kernel_scn<NP, false, false, true, false>(scn);
+    if (split) return ho ? step_kernel_scn<NP, true, true, false, false>(scn) : step_kernel_scn<NP, true, false, false, false>(scn);
+    return ho ? step_kernel_scn<NP, false, true, false, false>(scn) : step_kernel_scn<NP, false, false, false, false>(scn);
+}
+
+struct StepShape {
+    KernelFn fn;
+    int block, grid;
+    int work_threads;     // threads of a CTA that step envs: all but the courier warp
+    size_t smem;          // dynamic shared memory per CTA
+    int tile_off;         // StepParams.smem_tile_off: first float of the observation staging tiles
+    bool split, ho, courier;
+};
+
+// Launch shape of a step grid.  Three shapes run the same kernel body (qs_step.cuh):
+//  * split: 64-thread CTAs, a physics warp and an observer warp per 32 drones.  Splitting shortens one warp's dependency
+//    chain but adds work, so it only pays while the GPU has idle issue slots, i.e. up to about one physics warp per SM
+//    sub-partition (4 x the SM count).  QS_SPLIT=0/1 overrides the heuristic.
+//  * balanced: one CTA per SM, ceil(warps / SMs) worker warps each, so that every SM holds the same number of warps whatever
+//    the CTA scheduler does while two step grids overlap (the step ends with its slowest block).  With the per-block
+//    hand-over on a chained handle it gets a COURIER warp: one more warp that carries no envs and does the hand-over's flag
+//    traffic (acquire of the predecessor's state word, release of this block's state before the observation is built, the
+//    `done` word that orders the observation rows of consecutive steps).  A chained handle whose batch gives every SM at
+//    least two warps steps faster in this shape than in the split one.
+//  * otherwise: 64-thread single-warp CTAs over as many waves as it takes.
+// Host logic only; the one CUDA call is the occupancy query of a handle's first hand-over decision, whose error it returns.
+static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
+    const int NP = h->NP, sms = h->sms;
+    const bool dyn = h->st.dyn != nullptr, nz = h->nz_on;
+    const long long phys_warps = ((long long)h->cfg.num_envs * NP + 31) / 32;
+    const int wpc = (int)((phys_warps + sms - 1) / sms);          // worker warps per CTA of a balanced grid
+    const bool balance_fits = NP < 16 && wpc >= 2 && wpc * 32 <= QS_LB && (wpc * 32) % NP == 0;
+    const bool courier_fits = balance_fits && (wpc + 1) * 32 <= QS_LB;
+    const bool courier_shape = h->chained && !dyn && !nz && courier_fits;
+    const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
+    s.split = want_split && p.obs_stage && NP > 1 && !dyn && !nz && !h->obst_random;
+    const bool balanced = !s.split && balance_fits;
+    s.block = balanced ? wpc * 32 : 64;
+    s.work_threads = s.block;
+    const int envs_per_block = (s.split ? 32 : s.work_threads) / NP;
+    s.grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
+    size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
+    smem = (smem + 127) / 128 * 128;              // TMA sources are 128-byte aligned
+    s.tile_off = (int)(smem / sizeof(float));
+    if (p.obs_stage) smem += (size_t)(s.split ? 1 : s.work_threads / 32) * 32 * p.obs_dp * sizeof(float);
+    if (s.split) smem += (size_t)HAND_FLOATS * sizeof(float);
+    s.smem = smem;
+    const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
+    const bool scn = p.use_obst ? ticked_obst
+                                : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
+                                   p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
+    auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
+        KernelFn fn = nullptr;
+        dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
+        return fn;
+    };
+    // Per-block hand-over or grid-wide wait between step grids: decided at the handle's first step launch (QS_PDL=2 / 3 at
+    // qs_create forces the wait / the hand-over) and kept, so that every grid of a chain has the same shape.  The hand-over
+    // wins when a step grid needs more than one wave of CTAs, for the split shape, and with a courier warp.  With envs
+    // resetting in different steps, the reset of an env with a pillar table makes its block late; with the grid-wide wait
+    // every step pays that, with the hand-over only the block's own chain does.  Envs in lock-step otherwise favour the wait.
+    if (h->handover < 0) {
+        if (balanced) {
+            h->handover = courier_fits || h->cfg.use_obstacles;
+        } else {
+            int per_sm = 0;
+            QS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel(true, false, false), s.block, s.smem));
+            h->handover = s.split || (long long)s.grid > (long long)per_sm * sms || h->cfg.use_obstacles;
+        }
+    }
+    s.courier = balanced && courier_shape && h->handover == 1;
+    if (s.courier) s.block += 32;
+    // Shared-memory footprint of a balanced CTA.  Without a courier warp: 120 KB, i.e. one CTA per SM and never two CTAs of
+    // the same grid on one SM.  With it: 64 KB, so that the successor's CTA (whose block was released early) already runs
+    // on the SM while this one writes its observation rows, where registers allow (not the 9-warp CTAs, see QS_LB).
+    const size_t pad = (size_t)(s.courier ? 64 : 120) * 1024;
+    if (balanced && s.smem < pad) s.smem = pad;
+    // The hand-over kernels pay off only between step grids that follow each other directly; an unchained handle uses the
+    // grid-wide wait (formally safe after any predecessor) and never pre-fetches across the dependency wait.
+    s.ho = h->handover == 1 && h->chained && !dyn && !nz;
+    s.fn = kernel(s.ho, dyn, nz);
+    return QS_OK;
+}
+
 static int launch_pregen(QsHandle* h, cudaStream_t s);
 
 static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool obs_in_device_memory = true) {
     if (h->err_host && *(volatile int*)h->err_host != 0)
         return fail(QS_ERR_CUDA, "a per-block hand-over between step grids timed out earlier: the env state of this handle is "
                                  "not trustworthy any more (qs_handover_timeouts); destroy the handle");
-    // split kernel: physics warp + observer warp per 32 drones (QS_SPLIT=0/1 at qs_create overrides the heuristic)
-    // Splitting shortens one warp's dependency chain but adds work, so it only pays while the GPU has idle issue slots,
-    // i.e. up to about one physics warp per SM sub-partition (4 x the SM count).
-    if (h->pregen_every > 0) {
-        // next-episode records for the envs that consumed theirs (qs_pregen_kernel): every pregen_every step launches.  A
-        // captured graph repeats exactly the launches of its capture: a short graph captured between two generator launches
-        // and replayed forever never refills a record, and every auto-reset then generates its episode inside the step (same
-        // results; each such reset costs time, which the per-block hand-over mostly hides).  With QS_PREGEN_HEAD=1 every
-        // captured graph starts with a generator launch instead (which costs one more launch per replay).
-        bool due = (h->since_pregen += p_in.T) >= h->pregen_every;
-        static int head = -1;
-        if (head < 0) { const char* e = getenv("QS_PREGEN_HEAD"); head = e ? atoi(e) : 0; }
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        unsigned long long cid = 0;
-        if (head && cudaStreamGetCaptureInfo(s, &cs, &cid) == cudaSuccess && cs == cudaStreamCaptureStatusActive && cid != h->capture_id) {
-            h->capture_id = cid;
-            due = true;
-        }
-        if (due) {
-            int rcp = launch_pregen(h, s);
-            if (rcp != QS_OK) return rcp;
-        }
+    // Next-episode records for the envs that consumed theirs (qs_pregen_kernel): every pregen_every step launches.  A captured
+    // graph repeats exactly the launches of its capture: a short graph captured between two generator launches and replayed
+    // forever never refills a record, and every auto-reset then generates its episode inside the step (same results; each
+    // such reset costs time, which the per-block hand-over mostly hides).
+    if (h->pregen_every > 0 && (h->since_pregen += p_in.T) >= h->pregen_every) {
+        const int rc = launch_pregen(h, s);
+        if (rc != QS_OK) return rc;
     }
     StepParams p = p_in;
     choose_obs_writeout(h, p, obs_in_device_memory);
-    const long long phys_warps = ((long long)h->cfg.num_envs * h->NP + 31) / 32;
-    // A chained handle whose batch gives every SM at least two warps steps faster in the balanced shape with a courier warp
-    // (below) than in the split shape.
-    static int courier_env = -1;
-    if (courier_env < 0) { const char* e = getenv("QS_COURIER"); courier_env = e ? atoi(e) : 1; }
-    int sms = 0;
-    QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-    const int wpc_all = (int)((phys_warps + sms - 1) / sms);
-    const bool courier_shape = h->chained && courier_env && h->NP < 16 && h->st.dyn == nullptr && !h->nz_on && wpc_all >= 2 &&
-                               (wpc_all + 1) * 32 <= QS_LB && ((wpc_all * 32) % h->NP) == 0;
-    const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
-    const bool split = want_split && p.obs_stage && h->NP > 1 && h->st.dyn == nullptr && !h->nz_on && !h->obst_random;
-    // QS_BALANCE=1 (experiment): one CTA per SM, ceil(warps / SMs) warps each — every SM then holds the same number of warps
-    // whatever the CTA scheduler does while two step grids overlap (the timeline of the debug build showed SMs with 6 CTAs
-    // of 2 warps next to SMs with 2, and the step ends with the slowest block)
-    static int balance = -1;
-    if (balance < 0) { const char* e = getenv("QS_BALANCE"); balance = e ? atoi(e) : 1; }
-    int kBlock = split ? 64 : block_size();
-    if (h->NP >= 16 && kBlock > 128) kBlock = 128;          // launch bounds of the NP >= 16 instantiations
-    bool balanced = false;
-    if (balance && !split && h->NP < 16) {
-        const int wpc = wpc_all;
-        if (wpc >= 2 && wpc * 32 <= QS_LB && ((wpc * 32) % h->NP) == 0) { kBlock = wpc * 32; balanced = true; }
-    }
-    if (h->pdl_env == -2) {          // read once per handle
-        const char* e = getenv("QS_PDL");
-        const int m = e ? atoi(e) : -1;
-        h->pdl_env = (m < -1 || m > 4) ? -1 : m;
-    }
-    const int pdl_env = h->pdl_env;
-    // Balanced single-wave grids use the per-block hand-over with a COURIER warp (qs_step.cuh): one more warp per CTA that
-    // carries no envs and does the hand-over's flag traffic — acquire of the predecessor's state word, early release of
-    // this block's state (before the observation is built), the `done` word that orders the observation rows of consecutive
-    // steps.  QS_COURIER=0 switches it off.
-    if (h->handover < 0 && balanced)          // decided before the first launch so that every grid of a chain has the same shape
-        h->handover = pdl_env >= 0 ? (pdl_env == 3) : ((courier_env && kBlock + 32 <= QS_LB) || h->cfg.use_obstacles != 0);
-    const bool courier = balanced && courier_env && h->handover == 1 && h->chained && h->st.dyn == nullptr && !h->nz_on &&
-                         kBlock + 32 <= QS_LB;
-    if (courier) kBlock += 32;
-    p.courier = courier ? 1 : 0;
-    const int work_warps = kBlock / 32 - (courier ? 1 : 0);
-    const int envs_per_block = (split ? 32 : work_warps * 32) / h->NP;
-    const int grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
-    size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
-    smem = (smem + 127) / 128 * 128;              // TMA sources are 128-byte aligned
-    p.smem_tile_off = (int)(smem / sizeof(float));
-    if (p.obs_stage) smem += (size_t)(split ? 1 : work_warps) * 32 * p.obs_dp * sizeof(float);
-    if (split) smem += (size_t)HAND_FLOATS * sizeof(float);
-    // shared-memory footprint of a balanced CTA.  Without a courier warp: 120 KB, i.e. one CTA per SM and never two CTAs of
-    // the same grid on one SM.  With it: 64 KB, so that the successor's CTA (whose block was released early) already runs on
-    // the SM while this one writes its observation rows, where registers allow (not the 9-warp CTAs, see QS_LB).
-    // QS_BALANCE_KB overrides.
-    static int balance_kb = -1;
-    if (balance_kb < 0) { const char* e = getenv("QS_BALANCE_KB"); balance_kb = e ? atoi(e) : 0; }
-    const int pad_kb = balance_kb > 0 ? balance_kb : (courier ? 64 : 120);
-    if (balanced && smem < (size_t)pad_kb * 1024) smem = (size_t)pad_kb * 1024;
-    // Programmatic dependent launch between consecutive step grids (QS_PDL overrides; default -1 = choose per handle):
-    //   0 off; 1 grid-wide wait, trigger at kernel start (slower than 2); 2 grid-wide wait, trigger before the final
-    //   stores (faster than 0); 3 per-block hand-over, no grid-wide wait (qs_step.cuh).
-    // 3 wins when a step grid needs more than one wave of CTAs and for the split shape; for a single-wave grid whose
-    // warps run in lock-step anyway (c3) its acquire / release costs what the hidden launch latency saves, so 2 stays.
-    using KernelFn = void (*)(StepParams);
-    const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
-    const bool scn = p.use_obst ? ticked_obst
-                                : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
-                                   p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
-    KernelFn fn_wait = nullptr, fn_ho = nullptr;
-    int rc = dispatch_np(h->NP, [&](auto np) {
-        constexpr int NPv = decltype(np)::value;
-        if (split) {
-            fn_wait = scn ? (KernelFn)qs_step_kernel<NPv, true, true, false> : (KernelFn)qs_step_kernel<NPv, true, false, false>;
-            fn_ho = scn ? (KernelFn)qs_step_kernel<NPv, true, true, true> : (KernelFn)qs_step_kernel<NPv, true, false, true>;
-        } else {
-            fn_wait = scn ? (KernelFn)qs_step_kernel<NPv, false, true, false> : (KernelFn)qs_step_kernel<NPv, false, false, false>;
-            fn_ho = scn ? (KernelFn)qs_step_kernel<NPv, false, true, true> : (KernelFn)qs_step_kernel<NPv, false, false, true>;
-        }
-        return QS_OK;
-    });
+    StepShape sh;
+    const int rc = plan_step(h, p, sh);
     if (rc != QS_OK) return rc;
-    KernelFn fn_dyn = nullptr;
-    if (h->nz_on) {                       // custom sensor-noise model (with or without per-drone constants): same shape as DYN
-        const bool dyn = h->st.dyn != nullptr;
-        dispatch_np(h->NP, [&](auto np) {
-            constexpr int NPv = decltype(np)::value;
-            fn_dyn = dyn ? (scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, true, true>
-                                : (KernelFn)qs_step_kernel<NPv, false, false, false, true, true>)
-                         : (scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, false, true>
-                                : (KernelFn)qs_step_kernel<NPv, false, false, false, false, true>);
-            return QS_OK;
-        });
-    } else if (h->st.dyn != nullptr) {    // per-drone physical constants: single-warp shape, grid-wide wait
-        dispatch_np(h->NP, [&](auto np) {
-            constexpr int NPv = decltype(np)::value;
-            fn_dyn = scn ? (KernelFn)qs_step_kernel<NPv, false, true, false, true> : (KernelFn)qs_step_kernel<NPv, false, false, false, true>;
-            return QS_OK;
-        });
-    }
-    if (h->handover < 0) {
-        if (pdl_env >= 0) h->handover = pdl_env == 3;
-        else {
-            int per_sm = 0, sms = 0;
-            QS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn_ho, kBlock, smem));
-            QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-            // with envs resetting in different steps, the reset of an env with a pillar table makes its block late; with
-            // the grid-wide wait every step pays that, with the hand-over only the block's own chain does.  Envs in
-            // lock-step favour the grid-wide wait (QS_PDL=2 selects it).
-            h->handover = split || (long long)grid > (long long)per_sm * sms || h->cfg.use_obstacles != 0;
-        }
-    }
-    // The hand-over kernels pay off only between step grids that follow each other directly; an unchained handle uses
-    // the grid-wide wait (formally safe after any predecessor) and never pre-fetches across the dependency wait.
+    p.smem_tile_off = sh.tile_off;
+    p.courier = sh.courier ? 1 : 0;
     // inside qs_wrap_step the stream predecessor that counts is the block-chained wrapper kernel of the previous control step
     p.chained = (h->chained && (h->in_wrap_step ? h->last_was_wrap : h->last_was_step)) ? 1 : 0;
-    p.wrap_chain = (h->in_wrap_step && courier) ? 1 : 0;
-    static int poll_mode = -1;
-    if (poll_mode < 0) { const char* e = getenv("QS_POLL"); poll_mode = e ? atoi(e) : 40; }
-    p.poll_mode = poll_mode;
+    p.wrap_chain = (h->in_wrap_step && sh.courier) ? 1 : 0;
     h->step_wrap_chain = p.wrap_chain;
-    h->wrap_block = work_warps * 32;
+    h->wrap_block = sh.work_threads;
 #ifdef QS_TIMELINE
     if (!h->tl) { QS_CUDA(cudaMalloc((void**)&h->tl, sizeof(unsigned long long) * 64 * 4096 * 16)); QS_CUDA(cudaMemset(h->tl, 0, sizeof(unsigned long long) * 64 * 4096 * 16)); }
     p.tl = h->tl; p.tl_slot = h->tl_next; h->tl_next = (h->tl_next + 1) % 64;
 #endif
-    const bool use_ho = h->handover && h->chained && fn_dyn == nullptr;
-    const int pdl_mode = use_ho ? 3 : ((pdl_env >= 0 && pdl_env != 3) ? pdl_env : 2);
-    const bool use_pdl = pdl_mode != 0;
-    p.pdl_mode = pdl_mode;
+    // Programmatic dependent launch between consecutive step grids: a grid-wide-wait kernel lets the next grid launch just
+    // before its final stores (hides part of the launch latency of each step), a hand-over kernel once its blocks have taken
+    // their predecessors' state (qs_step.cuh).
     cudaLaunchConfig_t lc = {};
-    lc.gridDim = dim3(grid); lc.blockDim = dim3(kBlock); lc.dynamicSmemBytes = smem; lc.stream = s;
+    lc.gridDim = dim3(sh.grid); lc.blockDim = dim3(sh.block); lc.dynamicSmemBytes = sh.smem; lc.stream = s;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = attr; lc.numAttrs = use_pdl ? 1 : 0;
-    KernelFn fn = fn_dyn ? fn_dyn : (use_ho ? fn_ho : fn_wait);
-    if (smem + 1024 > 48 * 1024) QS_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      // + the kernel's static words
-    static int carve = -2;          // QS_CARVEOUT (experiment): preferred shared-memory carve-out in % for the step and wrapper kernels
-    if (carve == -2) { const char* e = getenv("QS_CARVEOUT"); carve = e ? atoi(e) : -1; }
-    if (carve >= 0) QS_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
-    const cudaError_t lerr = cudaLaunchKernelEx(&lc, fn, p);
+    lc.attrs = attr; lc.numAttrs = 1;
+    if (sh.smem + 1024 > 48 * 1024) QS_CUDA(cudaFuncSetAttribute((const void*)sh.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem));      // + the kernel's static words
+    const cudaError_t lerr = cudaLaunchKernelEx(&lc, sh.fn, p);
     if (lerr != cudaSuccess) return fail(QS_ERR_CUDA, std::string("cudaLaunchKernelEx: ") + cudaGetErrorString(lerr));
     QS_CUDA(cudaGetLastError());
     h->launches += 1;
@@ -558,7 +513,7 @@ static int launch_pregen(QsHandle* h, cudaStream_t s) {
 }
 
 static int launch_reset(QsHandle* h, const StepParams& p, cudaStream_t s) {
-    const int kBlock = block_size() > 128 ? 128 : block_size();
+    const int kBlock = 64;
     const int envs_per_block = kBlock / h->NP;
     const int grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
     const size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
@@ -611,11 +566,14 @@ extern "C" int qs_create(const QsConfig* cfg, int device, QsHandle** out) {
             return fail(QS_ERR_INVALID_ARG, "obstacle scenario: fewer free grid cells than drones");
     }
     QS_CUDA(cudaSetDevice(device));
+    int sms = 0;
+    QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     QsHandle* h = new (std::nothrow) QsHandle();
     if (!h) return fail(QS_ERR_INVALID_ARG, "out of host memory");
     memset(h, 0, sizeof(*h));
     h->cfg = *cfg;
     h->device = device;
+    h->sms = sms;
     h->NP = next_pow2(cfg->num_agents);
     h->K = K;
     h->S = cfg->obs_repr == 0 ? 18 : (cfg->obs_repr == 1 ? 19 : 24);
@@ -623,11 +581,12 @@ extern "C" int qs_create(const QsConfig* cfg, int device, QsHandle** out) {
     h->D = h->S + 6 * K + (cfg->use_obstacles ? 9 : 0);
     h->ep_len = (int)((double)cfg->ep_time / (0.005 * 2));      // quadrotor_single.py:158
     h->A = (long long)cfg->num_envs * cfg->num_agents;
-    {
+    {   // switches that tests use to force one launch shape (unset: automatic, plan_step)
         const char* e = getenv("QS_SPLIT");
         h->split_mode = e ? (atoi(e) != 0 ? 1 : 0) : -1;
-        h->handover = -1;
-        h->pdl_env = -2;
+        const char* pdl = getenv("QS_PDL");       // 2 grid-wide wait, 3 per-block hand-over between step grids
+        const int pm = pdl ? atoi(pdl) : -1;
+        h->handover = pm == 3 ? 1 : (pm == 2 ? 0 : -1);
         // next-episode generator cadence: an env consumes its record once per episode, so a quarter of an episode is ample
         const char* pg = getenv("QS_PREGEN");
         const bool dev_gen = cfg->scenario != QS_SCENARIO_HOST_TABLES;
@@ -637,7 +596,7 @@ extern "C" int qs_create(const QsConfig* cfg, int device, QsHandle** out) {
         const char* c = getenv("QS_CHAINED");
         h->chained = c ? (atoi(c) != 0) : 0;
         const char* b = getenv("QS_OBS_BULK");
-        h->bulk_mode = b ? atoi(b) : -1;          // 0 vector stores only, 2 linear bulk copies only, else automatic
+        h->bulk_mode = b ? atoi(b) : -1;          // 0 vector stores only, else automatic
     }
     h->a_pad = (h->A + 31) / 32 * 32;
     // QuadrotorEnvMulti defaults, quadrotor_multi.py:91-94
@@ -830,10 +789,6 @@ extern "C" int qs_wrap_apply(QsHandle* h, const float* actions_dev, const float*
 }
 
 static int launch_wrap(QsHandle* h, const float* actions_dev, const float* terms_dev, float* obs_dev, uint8_t* dones_dev, void* stream, bool chain) {
-    int rc = QS_OK;
-    static int probe = -1;                 // QS_WRAP_PROBE (tuning): 1 = skip the wrapper kernel, 2 = launch it without PDL
-    if (probe < 0) { const char* e = getenv("QS_WRAP_PROBE"); probe = e ? atoi(e) : 0; }
-    if (probe == 1) return QS_OK;
     WrapParams q;
     fill_params(h, q.sp);
     q.w = h->wrap;
@@ -853,17 +808,11 @@ static int launch_wrap(QsHandle* h, const float* actions_dev, const float* terms
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // launched behind the step grid's late trigger
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = attr; lc.numAttrs = probe == 2 ? 0 : 1;
+    lc.attrs = attr; lc.numAttrs = 1;
     using WrapFn = void (*)(WrapParams);
     WrapFn fn = nullptr;
-    rc = dispatch_np(h->NP, [&](auto np) { fn = (WrapFn)qs_wrap_kernel<decltype(np)::value>; return QS_OK; });
+    const int rc = dispatch_np(h->NP, [&](auto np) { fn = (WrapFn)qs_wrap_kernel<decltype(np)::value>; return QS_OK; });
     if (rc != QS_OK) return rc;
-    {
-        const char* e = getenv("QS_CARVEOUT");
-        if (e && atoi(e) >= 0) QS_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(e)));
-        const char* d = getenv("QS_WRAP_SMEM_KB");          // experiment: dummy dynamic shared memory of the wrapper kernel
-        if (e || d) { lc.dynamicSmemBytes = d ? (size_t)atoi(d) * 1024 : 0; if (lc.dynamicSmemBytes > 48 * 1024) QS_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lc.dynamicSmemBytes)); }
-    }
     const cudaError_t lerr = cudaLaunchKernelEx(&lc, fn, q);
     if (lerr != cudaSuccess) return fail(QS_ERR_CUDA, std::string("cudaLaunchKernelEx(wrap): ") + cudaGetErrorString(lerr));
     h->launches += 1;
@@ -1113,9 +1062,6 @@ extern "C" int qs_rollout(QsHandle* h, int num_steps, const float* actions_dev, 
     return launch_step(h, p, (cudaStream_t)stream);
 }
 
-#ifndef QS_ZERO_COPY_DEFAULT
-#define QS_ZERO_COPY_DEFAULT true          // the kernel reads / writes the page-locked host buffers itself: no copy launches
-#endif
 // true when the host pointer is page-locked (cudaHostAlloc / cudaHostRegister): DMA can use it directly.  `dev` receives the
 // device alias of a mapped buffer (or null).  The last few answers are cached: a rollout worker passes the same buffers on
 // every step, and the two driver queries per buffer cost more host time than enqueueing the step.
@@ -1177,17 +1123,15 @@ static int step_host_impl(QsHandle* h, const float* actions_host, float* obs_hos
     // outputs straight to, host memory — coalesced 128-bit stores over PCIe overlap the transfer with the step and save
     // the four copy launches (QS_ZERO_COPY=0 falls back to explicit copies).
     const char* zc_env = getenv("QS_ZERO_COPY");          // read per call: bench.py times both paths in one process
-    const bool zero_copy = zc_env ? atoi(zc_env) != 0 : QS_ZERO_COPY_DEFAULT;
+    const bool zero_copy = !zc_env || atoi(zc_env) != 0;
     if (zero_copy && pa && po && pr && pd && (!rew_terms_host || pt)) {
         const bool ok = da && dob && dr && dd && (!rew_terms_host || dt);
-        static int zc_bulk = -1;                           // QS_ZC_BULK=1 (experiment): observation tiles leave through the bulk-copy engine
-        if (zc_bulk < 0) { const char* e = getenv("QS_ZC_BULK"); zc_bulk = e ? atoi(e) : 0; }
         if (ok) {
             StepParams p;
             fill_params(h, p);
             p.actions = (const float4*)da;
             p.obs = (float*)dob; p.rewards = (float*)dr; p.dones = (uint8_t*)dd; p.rew_terms = (float*)dt;
-            int rc0 = launch_step(h, p, s, /*obs_in_device_memory=*/zc_bulk != 0);
+            int rc0 = launch_step(h, p, s, /*obs_in_device_memory=*/false);
             if (rc0 != QS_OK) return rc0;
             if (sync) QS_CUDA(cudaStreamSynchronize(s));
             return QS_OK;

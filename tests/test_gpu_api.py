@@ -332,7 +332,7 @@ def test_back_to_back_step_grids_equal_one_rollout(name, kw, E, dev_scn, pdl, ch
     what ONE launch that keeps the env block in registers gives, over several replays and across auto-resets."""
     from quad_swarm_rl_b200.engine import QuadSwarmEngine
     if pdl is not None:
-        monkeypatch.setenv('QS_PDL', pdl)           # read by each engine at its first step launch
+        monkeypatch.setenv('QS_PDL', pdl)           # read by each engine when it is created
     if 'split' in name:
         monkeypatch.setenv('QS_SPLIT', '1')         # a chained handle of this size would use the balanced shape with a courier warp
     if name.endswith('vector_stores'):
