@@ -115,6 +115,7 @@ struct StepParams {
     int ep_len, T, last_obs_only;
     float room_lo[3], room_hi[3];
     float col_thr, falloff_thr, obst_radius, obst_col_thr, obst_half_size;
+    float col_thr2, falloff_thr2, quad_arm;     // col_thr^2, falloff_thr^2, obst_col_thr - obst_half_size: kernel operands, not registers
     float grace_steps, final_steps, approach_metric;
     float rew[QS_NUM_REW_COEFF];
     uint32_t seed_lo, seed_hi;
@@ -254,6 +255,7 @@ __device__ __noinline__ float2 floor_random_yaw(RngKey key, int i, int sub) {
 // (calculate_torque_integrate_rotations_and_update_omega :497-566, room clip :360-367,
 //  floor_interaction_numba :569-639, compute_velocity_and_acceleration :642-649).
 // `cmd` is the RawControl output in [0,1]; the OU state s.ou is the thrust noise of this control step.
+template <bool FMA_FRICTION = false>
 __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], bool do_svd, const StepParams& p,
                                                  const RngKey& key, int i, int sub) {
     // motor lag on sqrt(thrust) + OU thrust noise (:504-517); linearity = 1 so thrust = thrust_max * cmds_damp
@@ -325,12 +327,14 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
 
     // floor contact / friction, threshold = arm (:569-639)
     float fx = s.R[2] * thrust_z, fy = s.R[5] * thrust_z;
-    const float fz = s.R[8] * thrust_z;
+    const float r22 = s.R[8], fz = r22 * thrust_z;
     if (s.pos[2] <= ARM) {
         s.pos[2] = ARM;
         if (fl & QS_FLAG_ON_FLOOR) {
             yaw_only(s.R);
-            const float fric = FLOOR_MU * (MASS * GRAV - fz);
+            // FMA_FRICTION: MASS * GRAV - fz with one rounding, written out.  The compiler fused it in these kernels before
+            // their register cap and no longer does; the other kernels keep the expression (and the compiler's choice) as it was.
+            const float fric = FLOOR_MU * (FMA_FRICTION ? __fmaf_rn(-r22, thrust_z, MASS * GRAV) : MASS * GRAV - fz);
             const float v2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1] + s.vel[2] * s.vel[2];
             if (v2 < EPS_DYN * EPS_DYN) {
                 // at rest: static friction eats the horizontal force (direction kept: cos/sin of atan2(fy, fx))

@@ -447,9 +447,19 @@ __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key
     }
 }
 
-// 8 worker warps + the courier: c3 / c5 (1024 physics warps) keep the courier on 132 SMs.  One such CTA per SM (~130-170
-// registers); two per SM (<= 112 registers) spill, and on H100 were slower on c5, c2 and the wrapped step.
+// Largest balanced CTA: 8 worker warps + the courier, or 9 worker warps without it (plan_step, quadswarm.cu).
 #define QS_LB 288
+// Register budget of the step instantiations.  The ones that can carry the courier warp (NP < 16, single-warp, per-block
+// hand-over, no DYN / NZ / SCN) get 128 registers per thread: plan_step gives c3 / c5 (1024 physics warps, 132 SMs on H100)
+// 256 CTAs of 4 workers + courier = 160 threads, and 160 x 128 = 20,480 registers let three such CTAs share an SM's 65,536,
+// so the successor's CTA of a block starts on an SM beside this step's (at 152 allocated registers, 288-thread CTAs of
+// 8 + 1 warps fit once: 43,776).  The bound is written as 512 threads per CTA (65,536 / 512 = 128) rather than (256, 2):
+// the same instantiations also run the 288-thread balanced CTAs.  The other instantiations (split, DYN, NZ, SCN with its
+// scenario generators, NP >= 16) keep one 288-thread (or 128-thread) CTA as their bound.
+template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN, bool NZ>
+__host__ __device__ constexpr bool courier_capable() { return NP < 16 && !SPLIT && !SCN && HO && !DYN && !NZ; }
+template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN, bool NZ>
+__host__ __device__ constexpr int step_max_threads() { return courier_capable<NP, SPLIT, SCN, HO, DYN, NZ>() ? 512 : (NP >= 16 ? 128 : QS_LB); }
 // named barriers of the split kernel (physics warp <-> observer warp, 64 threads).  Both warps use bar.sync: the
 // observer reaches barrier 1 first, the physics warp reaches barrier 2 first and has only its stores left to do.
 // Out of line on purpose: both warps then execute the SAME bar.sync instruction (what compute-sanitizer's synccheck
@@ -464,6 +474,18 @@ __device__ __noinline__ void bar_sync(int id) {
 __device__ __forceinline__ void named_sync(int id, int n) {
     __syncwarp();
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+// threads of the CTA and this thread's index, read where they are used (volatile: not kept in registers across the step
+// body of the courier-capable kernels, whose register budget is tight)
+__device__ __forceinline__ int block_threads() {
+    int n;
+    asm volatile("mov.u32 %0, %%ntid.x;" : "=r"(n));
+    return n;
+}
+__device__ __forceinline__ int thread_index() {
+    int n;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(n));
+    return n;
 }
 __device__ __forceinline__ void named_arrive(int id, int n) {
     __syncwarp();
@@ -583,7 +605,7 @@ __device__ __forceinline__ void hand_load(const float* hand, int lane, Agent& s,
 // NZ = true: the custom sensor-noise model (qs_set_sensor_noise, p.nz) instead of the compile-time 'default' set; the gyro
 // bias (p.gyro_bias, when that model is on) rides in registers across the steps of a launch.  Same shape as DYN.
 template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false, bool NZ = false>
-__global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const __grid_constant__ StepParams p) {
+__global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>()) qs_step_kernel(const __grid_constant__ StepParams p) {
     static_assert(!NZ || (!SPLIT && !HO), "the custom sensor-noise model runs in the single-warp shape with the grid-wide wait");
     extern __shared__ __align__(128) float2 s_obst[];
     __shared__ int s_late;          // courier launches: a block with a goal event behind the observation is released at its end
@@ -824,9 +846,8 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
     }
 
     bool goal_dirty = false;
-    bool stored_early = false, late_goal = false;      // state stores issued before the last observation; goal event after it
-    const float col_thr2 = p.col_thr * p.col_thr, falloff2 = p.falloff_thr * p.falloff_thr;
-    const float quad_arm = p.obst_col_thr - p.obst_half_size;                  // QuadrotorEnvMulti.quad_arm
+    bool late_goal = false;                            // goal event after the last observation (the single-warp shape stores the
+                                                       // state before it, at t = T - 1)
 
 #pragma unroll 1
     for (int t = 0; t < p.T; ++t) {
@@ -865,6 +886,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             const float4 av = (t == 0) ? av0 : __ldcs(p.actions + ((long long)t * A + a));
             act[0] = av.x; act[1] = av.y; act[2] = av.z; act[3] = av.w;
         }
+        av0 = make_float4(0.f, 0.f, 0.f, 0.f);         // used by the first step only: not live across the rest of the loop
         float cmd[4];
 #pragma unroll
         for (int m = 0; m < 4; ++m) cmd[m] = 0.5f * (clampf(act[m], -1.f, 1.f) + 1.f);    // RawControl.step, quadrotor_control.py:53-57
@@ -880,7 +902,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             const bool do_svd = ctr.svd_count >= SVD_PERIOD;
             if (do_svd) ctr.svd_count = 0;
             if (DYN) dynamics_substep_dyn(s, cmd, do_svd, p, key, i, sub, ph);
-            else dynamics_substep(s, cmd, do_svd, p, key, i, sub);
+            else dynamics_substep<courier_capable<NP, SPLIT, SCN, HO, DYN, NZ>()>(s, cmd, do_svd, p, key, i, sub);
         }
         if (SPLIT) {                                                   // positions are final from here on
             hand_store(s_hand, lane, s, s.vel);
@@ -899,6 +921,15 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         const float raw_crash = on_floor ? 1.0f : 0.0f;
         float reward = -SIM_DT * (p.rew[QS_REW_POS] * dist + p.rew[QS_REW_EFFORT] * raw_effort + p.rew[QS_REW_CRASH] * raw_crash +
                                   p.rew[QS_REW_ORIENT] * raw_orient + p.rew[QS_REW_SPIN] * raw_spin);
+        const long long ta = (long long)t * A + a;
+        if (valid && p.rew_terms) {              // the per-drone terms leave now: they are not kept live across the env part
+            float* tr = p.rew_terms + ta * QS_NUM_TERMS;
+            tr[QS_TERM_RAW_POS] = SIM_DT * -dist;
+            tr[QS_TERM_RAW_ACTION] = SIM_DT * -raw_effort;
+            tr[QS_TERM_RAW_CRASH] = SIM_DT * -raw_crash;
+            tr[QS_TERM_RAW_ORIENT] = SIM_DT * -raw_orient;
+            tr[QS_TERM_RAW_SPIN] = SIM_DT * -raw_spin;
+        }
         const int tick_before = ctr.tick;
         const int time_remain = p.ep_len - tick_before;
         ctr.tick = tick_before + 1;
@@ -921,9 +952,9 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
                             dz = s.pos[2] - shfl<NP>(s.pos[2], j);
                 const float d2 = dx * dx + dy * dy + dz * dz;
                 const bool other = (j != i) && valid;
-                if (other && d2 <= falloff2) {
+                if (other && d2 <= p.falloff_thr2) {
                     const float d = fsqrt(d2);
-                    if (d2 <= col_thr2) cur_col |= 1u << j;
+                    if (d2 <= p.col_thr2) cur_col |= 1u << j;
                     prox += pen_ratio * d + max_pen;
                 }
                 // the downwash cylinder (|rel_z| < 0.7, rel_xy < 0.1) lies inside the ball d^2 < 0.5: the z-axis
@@ -946,7 +977,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         int hit = -1;
         float dmin2 = 1e4f;                          // smallest squared centre distance to a pillar (prunes the SDF pass)
         if (p.use_obst) {
-            const float obst_thr = p.obst_random ? quad_arm + obst_r : p.obst_col_thr;
+            const float obst_thr = p.obst_random ? p.quad_arm + obst_r : p.obst_col_thr;
             const float obst_thr2 = obst_thr * obst_thr;
 #pragma unroll 4
             for (int m = p.M - 1; m >= 0; --m) {
@@ -1152,17 +1183,11 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         }
 
         // ================= outputs of this step =================
-        const long long ta = (long long)t * A + a;
         if (valid) {
             __stcs(p.rewards + ta, reward);
             __stcs(p.dones + ta, (uint8_t)(done ? 1 : 0));
             if (p.rew_terms) {
                 float* tr = p.rew_terms + ta * QS_NUM_TERMS;
-                tr[QS_TERM_RAW_POS] = SIM_DT * -dist;
-                tr[QS_TERM_RAW_ACTION] = SIM_DT * -raw_effort;
-                tr[QS_TERM_RAW_CRASH] = SIM_DT * -raw_crash;
-                tr[QS_TERM_RAW_ORIENT] = SIM_DT * -raw_orient;
-                tr[QS_TERM_RAW_SPIN] = SIM_DT * -raw_spin;
                 tr[QS_TERM_RAW_QUADCOL] = raw_quadcol;
                 tr[QS_TERM_PROXIMITY] = rew_prox;
                 tr[QS_TERM_RAW_QUADCOL_OBST] = raw_obst;
@@ -1255,14 +1280,13 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
             if (valid && dsum_dirty) st.slots[SL_DIST_SUMS * st.a_pad + a] = dsum;
             if (env_ok && i == 0) st.env_ctr[env] = make_int4(ctr.tick, ctr.step_count + 1, ctr.svd_count, ctr.episode_idx);
             if (gyro_model && valid) p.gyro_bias[a] = make_float4(gb.x, gb.y, gb.z, 0.f);
-            stored_early = true;
             if (has_courier) {
                 // Early hand-over: the successor block only needs this block's env STATE, which is complete now; the
                 // observation rows still to be written belong to this step's output arrays (the courier has made sure that
                 // the predecessor's rows are complete).  A goal event that must run after the observation (site B) keeps
                 // the state open: such a block (rare) is released at the end.
                 if (dev_scn && scn_ev && !kicked) *reinterpret_cast<volatile int*>(&s_late) = 1;
-                named_arrive(2, (int)blockDim.x);
+                named_arrive(2, block_threads());
                 // the rows of the previous instance are out (checked by the courier long ago: this does not spin in practice)
                 mbar_wait(&s_rows, 0);
             }
@@ -1284,12 +1308,13 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
                 // rows go to the warp's shared-memory tile, then out through the bulk-copy engine (or coalesced vector stores)
                 const int slot = (lane / NP) * p.N + i;               // row of this drone inside the warp's tile
                 if (p.obs_bulk && p.T > 1) bulk_drain();              // the previous step's copy has read the tile
-                write_observation<NP>(p, s, nvel, nz, i, valid, s_obst_env, dmin2, s_tile + slot * p.obs_dp, obst_r);
+                float* const tile = reinterpret_cast<float*>(s_obst) + p.smem_tile_off + (thread_index() >> 5) * (32 * p.obs_dp);  // = s_tile
+                write_observation<NP>(p, s, nvel, nz, i, valid, s_obst_env, dmin2, tile + slot * p.obs_dp, obst_r);
                 QS_TL(5);
-                const int env_first = blockIdx.x * envs_per_block + (threadIdx.x >> 5) * (32 / NP);
+                const int env_first = env - (thread_index() & 31) / NP;                   // first env of this warp
                 const int envs_here = min(32 / NP, p.E - env_first);
                 if (envs_here > 0)
-                    emit_observation_tile(p, s_tile, gbase + (long long)env_first * p.N * p.D, env_first * p.N,
+                    emit_observation_tile(p, tile, gbase + (long long)env_first * p.N * p.D, env_first * p.N,
                                           p.last_obs_only ? 0 : t, envs_here * p.N, lane);
                 __syncwarp();
             } else {
@@ -1317,7 +1342,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
 
     if (!HO) asm volatile("griddepcontrol.launch_dependents;");                 // late trigger: overlap only the launch latency
     QS_TL(6);
-    if (!stored_early || late_goal) {
+    if (SPLIT || late_goal) {
         if (valid) store_agent(st, a, s, goal_dirty);
         if (valid && dsum_dirty) st.slots[SL_DIST_SUMS * st.a_pad + a] = dsum;
         if (env_ok && i == 0) st.env_ctr[env] = make_int4(ctr.tick, ctr.step_count, ctr.svd_count, ctr.episode_idx);
@@ -1328,7 +1353,7 @@ __global__ void __launch_bounds__(NP >= 16 ? 128 : QS_LB) qs_step_kernel(const _
         else bulk_drain();                            // shared memory must outlive the bulk copy's reads
     }
     if (HO) {
-        if (has_courier) named_arrive(3, (int)blockDim.x);
+        if (has_courier) named_arrive(3, block_threads());
         else {
             if (SPLIT) bar_sync(4); else __syncthreads();
             if (threadIdx.x == 0) handover_release(st.ready + blockIdx.x);

@@ -30,6 +30,7 @@ struct QsHandle {
     int64_t launches;
     int split_mode;       // -1 auto, 0 single-warp kernel, 1 split kernel (QS_SPLIT)
     int handover;         // -1 not decided yet, 0 grid-wide wait between step grids, 1 per-block hand-over (plan_step; QS_PDL)
+    int courier_wpc;      // 0 not decided yet, else worker warps per CTA of a grid with the courier warp (courier_workers)
     int obst_random, n_obst_counts, n_obst_radii;
     int obst_counts[QS_MAX_OBST_CHOICES];
     float obst_radii[QS_MAX_OBST_CHOICES];
@@ -108,6 +109,9 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.obst_radius = (float)(c.obst_size / 2.0);
     p.obst_col_thr = (float)(arm + c.obst_size / 2.0);           // obstacles/utils.py:33
     p.obst_half_size = (float)(c.obst_size / 2.0);
+    p.col_thr2 = p.col_thr * p.col_thr;                          // float products / difference, as the kernel formed them
+    p.falloff_thr2 = p.falloff_thr * p.falloff_thr;
+    p.quad_arm = p.obst_col_thr - p.obst_half_size;              // QuadrotorEnvMulti.quad_arm
     p.grace_steps = 150.f;                                       // 1.5 * control_freq, quadrotor_multi.py:146
     p.final_steps = 500.f;                                       // 5.0 * control_freq, quadrotor_multi.py:150
     p.approach_metric = c.approch_goal_metric;
@@ -375,6 +379,33 @@ struct StepShape {
     bool split, ho, courier;
 };
 
+// Shared-memory footprint of a CTA with the courier warp: 3 x (64 KB + the 1 KB the SM reserves per CTA) fit the 228 KB
+// of an H100 SM.
+static const size_t COURIER_SMEM = (size_t)64 * 1024;
+
+// Worker warps per CTA of a chained grid with the courier warp.  ceil(warps / SMs) (`wpc_even`) gives every SM one CTA of
+// a step; but the early hand-over pays only if the successor's CTA of a block can start on an SM while the block still writes
+// its observation rows.  So the count is the largest one, at most wpc_even, whose CTAs let every SM hold its share of a step
+// grid plus one more CTA, by the kernel's occupancy; wpc_even when none does.  c3 / c5 (1024 physics warps, 132 SMs):
+// 8 workers + courier = 288 threads at <= 128 registers fit once per SM (36,864 of 65,536 registers); 4 workers + courier
+// = 160 threads fit three times (3 x 20,480), so a 256-CTA grid (at most two per SM) leaves room for the successor's CTA.
+// c2 (256 warps) keeps 2 workers.  Decided at the handle's first launch in this shape (one occupancy query per candidate,
+// no CUDA call afterwards) and kept, like the hand-over decision.
+static int courier_workers(QsHandle* h, KernelFn fn, int wpc_even) {
+    if (h->courier_wpc > 0) return QS_OK;
+    QS_CUDA(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COURIER_SMEM));
+    int pick = wpc_even;
+    for (int w = wpc_even; w >= 2; --w) {
+        int per_sm = 0;
+        QS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, (w + 1) * 32, COURIER_SMEM));
+        const int envs_per_block = w * 32 / h->NP;
+        const long long grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
+        if (per_sm >= (grid + h->sms - 1) / h->sms + 1) { pick = w; break; }
+    }
+    h->courier_wpc = pick;
+    return QS_OK;
+}
+
 // Launch shape of a step grid.  Three shapes run the same kernel body (qs_step.cuh):
 //  * split: 64-thread CTAs, a physics warp and an observer warp per 32 drones.  Splitting shortens one warp's dependency
 //    chain but adds work, so it only pays while the GPU has idle issue slots, i.e. up to about one physics warp per SM
@@ -384,20 +415,39 @@ struct StepShape {
 //    hand-over on a chained handle it gets a COURIER warp: one more warp that carries no envs and does the hand-over's flag
 //    traffic (acquire of the predecessor's state word, release of this block's state before the observation is built, the
 //    `done` word that orders the observation rows of consecutive steps).  A chained handle whose batch gives every SM at
-//    least two warps steps faster in this shape than in the split one.
+//    least two warps steps faster in this shape than in the split one.  The courier shape takes fewer worker warps per CTA
+//    where that lets an SM hold a CTA of the next step beside those of this one (courier_workers): c3 / c5 run 256 CTAs of
+//    4 workers + courier (160 threads, up to three per SM) instead of 128 CTAs of 8 + 1.
 //  * otherwise: 64-thread single-warp CTAs over as many waves as it takes.
-// Host logic only; the one CUDA call is the occupancy query of a handle's first hand-over decision, whose error it returns.
+// Host logic only; the CUDA calls are the occupancy queries of a handle's first hand-over and courier decisions, whose
+// errors it returns.
 static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const int NP = h->NP, sms = h->sms;
     const bool dyn = h->st.dyn != nullptr, nz = h->nz_on;
     const long long phys_warps = ((long long)h->cfg.num_envs * NP + 31) / 32;
-    const int wpc = (int)((phys_warps + sms - 1) / sms);          // worker warps per CTA of a balanced grid
+    int wpc = (int)((phys_warps + sms - 1) / sms);          // worker warps per CTA of a balanced grid
     const bool balance_fits = NP < 16 && wpc >= 2 && wpc * 32 <= QS_LB && (wpc * 32) % NP == 0;
     const bool courier_fits = balance_fits && (wpc + 1) * 32 <= QS_LB;
     const bool courier_shape = h->chained && !dyn && !nz && courier_fits;
     const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
     s.split = want_split && p.obs_stage && NP > 1 && !dyn && !nz && !h->obst_random;
     const bool balanced = !s.split && balance_fits;
+    const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
+    const bool scn = p.use_obst ? ticked_obst
+                                : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
+                                   p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
+    auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
+        KernelFn fn = nullptr;
+        dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
+        return fn;
+    };
+    // A balanced grid that will carry the courier warp (the hand-over is, or will be, chosen below): its worker warps per CTA
+    // come from the kernel's occupancy (courier_workers), and the env -> block mapping follows them.
+    if (balanced && courier_shape && h->handover != 0) {
+        const int rc = courier_workers(h, kernel(true, false, false), wpc);
+        if (rc != QS_OK) return rc;
+        wpc = h->courier_wpc;
+    }
     s.block = balanced ? wpc * 32 : 64;
     s.work_threads = s.block;
     const int envs_per_block = (s.split ? 32 : s.work_threads) / NP;
@@ -408,15 +458,6 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     if (p.obs_stage) smem += (size_t)(s.split ? 1 : s.work_threads / 32) * 32 * p.obs_dp * sizeof(float);
     if (s.split) smem += (size_t)HAND_FLOATS * sizeof(float);
     s.smem = smem;
-    const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
-    const bool scn = p.use_obst ? ticked_obst
-                                : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
-                                   p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
-    auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
-        KernelFn fn = nullptr;
-        dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
-        return fn;
-    };
     // Per-block hand-over or grid-wide wait between step grids: decided at the handle's first step launch (QS_PDL=2 / 3 at
     // qs_create forces the wait / the hand-over) and kept, so that every grid of a chain has the same shape.  The hand-over
     // wins when a step grid needs more than one wave of CTAs, for the split shape, and with a courier warp.  With envs
@@ -434,9 +475,10 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     s.courier = balanced && courier_shape && h->handover == 1;
     if (s.courier) s.block += 32;
     // Shared-memory footprint of a balanced CTA.  Without a courier warp: 120 KB, i.e. one CTA per SM and never two CTAs of
-    // the same grid on one SM.  With it: 64 KB, so that the successor's CTA (whose block was released early) already runs
-    // on the SM while this one writes its observation rows, where registers allow (not the 9-warp CTAs, see QS_LB).
-    const size_t pad = (size_t)(s.courier ? 64 : 120) * 1024;
+    // the same grid on one SM.  With it: COURIER_SMEM, which lets the three CTAs that registers allow share an SM (see
+    // courier_workers), so that the successor's CTA (whose block was released early) already runs on the SM while this one
+    // writes its observation rows.
+    const size_t pad = s.courier ? COURIER_SMEM : (size_t)120 * 1024;
     if (balanced && s.smem < pad) s.smem = pad;
     // The hand-over kernels pay off only between step grids that follow each other directly; an unchained handle uses the
     // grid-wide wait (formally safe after any predecessor) and never pre-fetches across the dependency wait.

@@ -82,6 +82,20 @@ for k in (5, 12):
     print(f'step {k + 2}: blocks per SM histogram {np.bincount(cnt)[1:].tolist()} | median waited->exit by #blocks on the SM: ' +
           ' '.join(f'{c}:{np.median(dur[k][per == c]):.2f}(n={int((per == c).sum())})' for c in np.unique(per)))
 print('waited->exit percentiles (us) 50/90/99/max:', np.round(np.percentile(dur, [50, 90, 99, 100]), 2))
+# SM time by what the SM holds, between the first entry of the 2nd and the last exit of the next-to-last recorded step:
+# no CTA, one CTA that still waits for its predecessor (entry -> waited), one working CTA, two or more CTAs
+w0, w1 = d[1, :, 0].min(), d[-2, :, 7].max()
+share = np.zeros(4)
+for s_ in np.unique(sm):
+    m = sm == s_
+    ent, wt, ex = d[:, :, 0][m], d[:, :, 1][m], d[:, :, 7][m]
+    pts = np.unique(np.clip(np.concatenate([ent, wt, ex, [w0, w1]]), w0, w1))
+    mid, ln = (pts[:-1] + pts[1:]) / 2, np.diff(pts)
+    res = ((ent[None] <= mid[:, None]) & (ex[None] > mid[:, None])).sum(1)
+    waiting = ((ent[None] <= mid[:, None]) & (wt[None] > mid[:, None])).sum(1)
+    share += [ln[res == 0].sum(), ln[(res == 1) & (waiting == 1)].sum(), ln[(res == 1) & (waiting == 0)].sum(), ln[res >= 2].sum()]
+share /= share.sum()
+print('SM time shares: idle {:.3f} | one CTA, waiting for its predecessor {:.3f} | one CTA, working {:.3f} | two or more CTAs {:.3f}'.format(*share))
 slow = np.argsort(dur[5])[-8:]
 print('slowest blocks of step 7:', [(int(b), int(sm[5][b]), round(float(dur[5][b]), 2), np.round(np.diff(d[5, b, 1:8]), 2).tolist()) for b in slow])
 # reset path of the blocks that had one (stamps 9..11: start of the episode-end branch, after reset_env, after the redraw)
