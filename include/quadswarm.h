@@ -295,6 +295,21 @@ int qs_set_gyro_bias(QsHandle* h, const uint8_t* env_mask_dev, const float* bias
  * with QS_ERR_INVALID_ARG (the reference fixes the option in its constructor).  Works in every step shape. */
 int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega_max);
 
+/* Dynamics path — replaces QuadrotorEnvMulti(use_numba=False) (quadrotor_multi.py:67 -> QuadrotorSingle -> QuadrotorDynamics,
+ * quadrotor_dynamics.py:211-214): enable = 1 steps the physics of the reference's numpy path, QuadrotorDynamics.step1 +
+ * floor_interaction (:225-346, :389-457), instead of its njit path (step1_numba + floor_interaction_numba, :348-383, :569-639),
+ * which is the default.  Only the floor model differs:
+ *   - floor threshold and snap height 0.05 for every drone (:75, :392-393), not the drone's arm (:378);
+ *   - at rest only when all three velocity components are exactly 0 (:406), not |vel| < 1e-6 (:586);
+ *   - sliding friction (cos, sin)(atan2(-vy, -vx)), subtracted (:419-422): it pushes the drone along its velocity;
+ *   - an upside-down first contact re-draws randyaw() until the body x-axis points within 60 deg of the origin (:434-437),
+ *     at most 64 tries (draw site 23), instead of one uniform yaw (:616-619).
+ * The thrust noise and sensor noise keep their keyed draws (same distributions in both paths); the per-drone constants of
+ * qs_set_dynamics apply their rotor drag in both paths.  enable = 0 restores the default.  Call after qs_create and before the
+ * first qs_reset / qs_step; later calls fail with QS_ERR_INVALID_ARG (the reference fixes use_numba in its constructor).
+ * Works in every step shape. */
+int qs_set_numpy_dynamics(QsHandle* h, int enable);
+
 /* flag bits in agent_u32[.,0] */
 #define QS_FLAG_ON_FLOOR (1u << 0)
 #define QS_FLAG_CRASHED_FLOOR (1u << 1)

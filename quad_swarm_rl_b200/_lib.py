@@ -101,6 +101,7 @@ EXPORTS = {
     'qs_get_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_init_random_state': (C.c_int, [C.c_void_p, C.c_int, C.c_float, C.c_float]),
+    'qs_set_numpy_dynamics': (C.c_int, [C.c_void_p, C.c_int]),
     'qs_wrap_enable': (C.c_int, [C.c_void_p, C.POINTER(QsWrapConfig)]),
     'qs_wrap_step': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_wrap_apply': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

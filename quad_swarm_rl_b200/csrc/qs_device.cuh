@@ -36,6 +36,14 @@ constexpr float ARM = 0.04596194077712559f;       // quadrotor_dynamics.py:158 (
 constexpr float MOTOR_TAU_UP = 0.13333244445037035f, MOTOR_TAU_DOWN = 0.13333244445037035f;
 constexpr float OMEGA_MAX = 40.0f;
 constexpr float FLOOR_MU = 0.6f;
+// QS_NUMPY_DYNAMICS = 1 (set by qs_step_npy.cu only): the floor model of the reference's numpy path (use_numba=False;
+// QuadrotorDynamics.floor_interaction, quadrotor_dynamics.py:389-457) in dynamics_substep() / dynamics_substep_dyn().
+#ifndef QS_NUMPY_DYNAMICS
+#define QS_NUMPY_DYNAMICS 0
+#endif
+#if QS_NUMPY_DYNAMICS
+constexpr float FLOOR_THRESHOLD_NP = 0.05f;       // floor threshold and snap height of the numpy path, every model (:75)
+#endif
 constexpr float SIM_DT = 0.005f;                  // quadrotor_single.py:157
 constexpr float CONTROL_DT = 0.01f;               // quadrotor_multi.py:83
 constexpr int SIM_STEPS = 2;                      // quadrotor_single.py:102
@@ -251,10 +259,24 @@ __device__ __noinline__ float2 floor_random_yaw(RngKey key, int i, int sub) {
     return make_float2(c, s);
 }
 
+#if QS_NUMPY_DYNAMICS
+__device__ __noinline__ float2 floor_yaw_numpy(RngKey key, int i, int sub, float x, float y);      // below
+
+// Sliding-friction direction of the numpy path, (cos, sin)(atan2(-vy, -vx)) (quadrotor_dynamics.py:419-422), from the njit
+// path's (ca, sa) = v_xy / |v_xy|: the friction is subtracted along the velocity there, so it pushes the drone on.  With no
+// horizontal velocity atan2 sees signed zeros: atan2(-0, -0) = -pi for vx = +0 (direction (-1, 0)), atan2(-0, +0) = -0 for
+// vx = -0 (direction (1, 0)); the sin(-pi) = -1.2e-16 of the first is dropped.
+__device__ __forceinline__ void friction_dir_numpy(float vx, float h2, float& ca, float& sa) {
+    if (h2 > 0.f) { ca = -ca; sa = -sa; }
+    else ca = copysignf(1.f, -vx);
+}
+#endif
+
 // One 5 ms physics sub-step of the njit path: step1_numba, quadrotor_dynamics.py:348-383
 // (calculate_torque_integrate_rotations_and_update_omega :497-566, room clip :360-367,
 //  floor_interaction_numba :569-639, compute_velocity_and_acceleration :642-649).
 // `cmd` is the RawControl output in [0,1]; the OU state s.ou is the thrust noise of this control step.
+// QS_NUMPY_DYNAMICS: the floor model of the numpy path instead (floor_interaction, :389-457).
 template <bool FMA_FRICTION = false>
 __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], bool do_svd, const StepParams& p,
                                                  const RngKey& key, int i, int sub) {
@@ -325,18 +347,28 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
     if (px != s.pos[0] || py != s.pos[1]) fl |= QS_FLAG_CRASHED_WALL;
     if (pz > s.pos[2]) fl |= QS_FLAG_CRASHED_CEILING;
 
-    // floor contact / friction, threshold = arm (:569-639)
+    // floor contact / friction, threshold = arm (:569-639).  Numpy path: threshold 0.05 (:75), exact at-rest test (:406),
+    // friction along the velocity (:419-422), re-drawn landing yaw (:434-437)
+#if QS_NUMPY_DYNAMICS
+    constexpr float floor_z = FLOOR_THRESHOLD_NP;
+#else
+    constexpr float floor_z = ARM;
+#endif
     float fx = s.R[2] * thrust_z, fy = s.R[5] * thrust_z;
     const float r22 = s.R[8], fz = r22 * thrust_z;
-    if (s.pos[2] <= ARM) {
-        s.pos[2] = ARM;
+    if (s.pos[2] <= floor_z) {
+        s.pos[2] = floor_z;
         if (fl & QS_FLAG_ON_FLOOR) {
             yaw_only(s.R);
             // FMA_FRICTION: MASS * GRAV - fz with one rounding, written out.  The compiler fused it in these kernels before
             // their register cap and no longer does; the other kernels keep the expression (and the compiler's choice) as it was.
             const float fric = FLOOR_MU * (FMA_FRICTION ? __fmaf_rn(-r22, thrust_z, MASS * GRAV) : MASS * GRAV - fz);
+#if QS_NUMPY_DYNAMICS
+            if (s.vel[0] == 0.f && s.vel[1] == 0.f && s.vel[2] == 0.f) {       // :406
+#else
             const float v2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1] + s.vel[2] * s.vel[2];
             if (v2 < EPS_DYN * EPS_DYN) {
+#endif
                 // at rest: static friction eats the horizontal force (direction kept: cos/sin of atan2(fy, fx))
                 const float f2 = fx * fx + fy * fy;
                 const float fm = fsqrt(f2);
@@ -355,14 +387,21 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
                     const float inv = frsqrt(h2);
                     ca = s.vel[0] * inv; sa = s.vel[1] * inv;
                 }
+#if QS_NUMPY_DYNAMICS
+                friction_dir_numpy(s.vel[0], h2, ca, sa);
+#endif
                 fx -= ca * fric; fy -= sa * fric;
             }
         } else {
             fl |= QS_FLAG_ON_FLOOR | QS_FLAG_CRASHED_FLOOR;
             s.vel[0] = s.vel[1] = s.vel[2] = 0.f;
             s.om[0] = s.om[1] = s.om[2] = 0.f;
-            if (s.R[8] < 0.f) {                         // upside down: random yaw (:616-619)
+            if (s.R[8] < 0.f) {                         // upside down: random yaw (:616-619; numpy path :434-437)
+#if QS_NUMPY_DYNAMICS
+                const float2 cs = floor_yaw_numpy(key, i, sub, s.pos[0], s.pos[1]);
+#else
                 const float2 cs = floor_random_yaw(key, i, sub);
+#endif
                 s.R[0] = cs.x; s.R[1] = -cs.y; s.R[2] = 0.f; s.R[3] = cs.y; s.R[4] = cs.x; s.R[5] = 0.f;
                 s.R[6] = 0.f; s.R[7] = 0.f; s.R[8] = 1.f;
             } else {
@@ -414,6 +453,7 @@ __device__ __forceinline__ void load_phys(const float4* rows, long long a, Phys&
 // One 5 ms physics sub-step with per-drone constants: the njit path as in dynamics_substep() above — general motor
 // asymmetry / linearity / propeller positions / damping — plus the rotor-drag and rolling-moment term that only the
 // reference's numpy path has (step1, quadrotor_dynamics.py:256-289; all shipped models have C_drag = C_roll = 0).
+// QS_NUMPY_DYNAMICS: the numpy path's floor model, as in dynamics_substep().
 __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], bool do_svd, const StepParams& p, const RngKey& key,
                                                   int i, int sub, const Phys& ph) {
     float thr[4];
@@ -509,18 +549,27 @@ __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], 
     if (px != s.pos[0] || py != s.pos[1]) fl |= QS_FLAG_CRASHED_WALL;
     if (pz > s.pos[2]) fl |= QS_FLAG_CRASHED_CEILING;
 
-    // force in the world frame: R (thrust + rotor drag), floor contact with threshold = this drone's arm (:378)
+    // force in the world frame: R (thrust + rotor drag), floor contact with threshold = this drone's arm (:378), or 0.05
     float fx = s.R[0] * drag_fx + s.R[1] * drag_fy + s.R[2] * (thrust_z + drag_fz);
     float fy = s.R[3] * drag_fx + s.R[4] * drag_fy + s.R[5] * (thrust_z + drag_fz);
     const float fz = s.R[6] * drag_fx + s.R[7] * drag_fy + s.R[8] * (thrust_z + drag_fz);
     const float keep = 1.f - ph.vel_damp;
-    if (s.pos[2] <= ph.arm) {
-        s.pos[2] = ph.arm;
+#if QS_NUMPY_DYNAMICS
+    const float floor_z = FLOOR_THRESHOLD_NP;
+#else
+    const float floor_z = ph.arm;
+#endif
+    if (s.pos[2] <= floor_z) {
+        s.pos[2] = floor_z;
         if (fl & QS_FLAG_ON_FLOOR) {
             yaw_only(s.R);
             const float fric = FLOOR_MU * (ph.mass * GRAV - fz);
+#if QS_NUMPY_DYNAMICS
+            if (s.vel[0] == 0.f && s.vel[1] == 0.f && s.vel[2] == 0.f) {
+#else
             const float v2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1] + s.vel[2] * s.vel[2];
             if (v2 < EPS_DYN * EPS_DYN) {
+#endif
                 const float fm = fsqrt(fx * fx + fy * fy);
                 const float mag = fmaxf(fm - fric, 0.f);
                 if (fm > 0.f) {
@@ -536,6 +585,9 @@ __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], 
                     const float inv = frsqrt(h2);
                     ca = s.vel[0] * inv; sa = s.vel[1] * inv;
                 }
+#if QS_NUMPY_DYNAMICS
+                friction_dir_numpy(s.vel[0], h2, ca, sa);
+#endif
                 fx -= ca * fric; fy -= sa * fric;
             }
         } else {
@@ -543,7 +595,11 @@ __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], 
             s.vel[0] = s.vel[1] = s.vel[2] = 0.f;
             s.om[0] = s.om[1] = s.om[2] = 0.f;
             if (s.R[8] < 0.f) {
+#if QS_NUMPY_DYNAMICS
+                const float2 cs = floor_yaw_numpy(key, i, sub, s.pos[0], s.pos[1]);
+#else
                 const float2 cs = floor_random_yaw(key, i, sub);
+#endif
                 s.R[0] = cs.x; s.R[1] = -cs.y; s.R[2] = 0.f; s.R[3] = cs.y; s.R[4] = cs.x; s.R[5] = 0.f;
                 s.R[6] = 0.f; s.R[7] = 0.f; s.R[8] = 1.f;
             } else {
@@ -1043,5 +1099,25 @@ __device__ __noinline__ InitState random_init_state(RngKey key, int i, float vel
     o.R[6] = fwd.z; o.R[7] = left.z; o.R[8] = up.z;
     return o;
 }
+
+#if QS_NUMPY_DYNAMICS
+// The landing yaw of the numpy path (floor_interaction, quadrotor_dynamics.py:434-437): randyaw() is re-drawn until the body
+// x-axis points within 60 deg of the origin, seen from the snapped position (x, y) — to_xyhat(-pos), quad_utils.py:120-124.
+// Capped at RESET_YAW_MAX_TRIES like reset_pose (DESIGN, deviations).
+__device__ __noinline__ float2 floor_yaw_numpy(RngKey key, int i, int sub, float x, float y) {
+    float hx = -x, hy = -y;
+    const float n = sqrtf(hx * hx + hy * hy);
+    if (!(n < 0.00001f)) { hx /= n; hy /= n; }
+    float sn = 0.f, cs = 1.f;
+    float4 u = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+    for (int k = 0; k < RESET_YAW_MAX_TRIES; ++k) {
+        if ((k & 3) == 0) u = rng_uniform4(key, SITE_FLOOR_YAW_NP, i, sub, k >> 2);
+        sincosf(-PI_F + (PI_F - (-PI_F)) * u4_word(u, k & 3), &sn, &cs);
+        if (cs * hx + sn * hy >= 0.5f) break;          // rot[:, 0] = (cos, sin, 0)
+    }
+    return make_float2(cs, sn);
+}
+#endif
 
 }  // namespace qs

@@ -49,9 +49,12 @@ enum Site : uint32_t {
     // episode-keyed like SITE_SPAWN_U.  Full-precision draws; CPU twin: oracle/init_state_oracle.py.
     SITE_INIT_U = 21,       // (i)   uniforms v0..2 vel direction, v3 vel magnitude, v4..6 omega direction, v7 omega magnitude
     SITE_INIT_N = 22,       // (i)   normals v0..2 up, v[4(t+1)..4(t+1)+2] fwd of try t        rand_uniform_rot3d, quad_utils.py:94-104
+    // Upside-down first floor contact of the numpy dynamics path (qs_set_numpy_dynamics; floor_interaction,
+    // quadrotor_dynamics.py:434-437), step-keyed like SITE_FLOOR_YAW.  CPU twin: oracle/numpy_path_oracle.py.
+    SITE_FLOOR_YAW_NP = 23, // (i,j) uniforms v[k], j = sub-step, k = rejection try of randyaw()
 };
 
-constexpr int RESET_YAW_MAX_TRIES = 64;
+constexpr int RESET_YAW_MAX_TRIES = 64;     // also caps the SITE_FLOOR_YAW_NP loop (reference: unbounded; p(re-draw) = 2/3)
 constexpr int INIT_ROT_MAX_TRIES = 16;      // fwd re-draws of rand_uniform_rot3d (reference: unbounded; p(re-draw) ~ 2.5 %)
 
 struct RngKey {

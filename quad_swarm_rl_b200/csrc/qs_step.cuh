@@ -604,6 +604,8 @@ __device__ __forceinline__ void hand_load(const float* hand, int lane, Agent& s,
 // instantiated for the single-warp shape with the grid-wide wait.
 // NZ = true: the custom sensor-noise model (qs_set_sensor_noise, p.nz) instead of the compile-time 'default' set; the gyro
 // bias (p.gyro_bias, when that model is on) rides in registers across the steps of a launch.  Same shape as DYN.
+// qs_step_npy.cu compiles this kernel once more, as qs_step_kernel_npy, with the floor model of the reference's numpy path
+// (QS_NUMPY_DYNAMICS, qs_set_numpy_dynamics).
 template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false, bool NZ = false>
 __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>()) qs_step_kernel(const __grid_constant__ StepParams p) {
     static_assert(!NZ || (!SPLIT && !HO), "the custom sensor-noise model runs in the single-warp shape with the grid-wide wait");

@@ -55,9 +55,11 @@ struct QsHandle {
     bool nz_on;           // qs_set_sensor_noise: the custom sensor-noise model (NZ kernels)
     NoiseModel nz;
     float4* gyro_bias;    // [A], allocated when the gyro bias model is on
-    bool started;         // a reset or step has been enqueued: the noise model and the initial-state mode are fixed from here on
+    bool started;         // a reset or step has been enqueued: the noise model, the initial-state mode and the dynamics path
+                          // are fixed from here on
     int init_random;      // qs_set_init_random_state
     float init_vel_max, init_omega_max;
+    int numpy_dyn;        // qs_set_numpy_dynamics
     cudaStream_t last_stream;   // stream of the most recent asynchronous call of this handle
     bool async_pending;
     // staging for the *_host entry points (pinned host + device mirrors)
@@ -353,21 +355,11 @@ static int dispatch_np(int NP, F&& f) {
     return fail(QS_ERR_UNSUPPORTED, "num_agents > 32 is not supported by this build");
 }
 
-using KernelFn = void (*)(StepParams);
+#include "qs_step_select.cuh"
 
-template <int NP, bool SPLIT, bool HO, bool DYN, bool NZ>
-static KernelFn step_kernel_scn(bool scn) {
-    return scn ? (KernelFn)qs_step_kernel<NP, SPLIT, true, HO, DYN, NZ> : (KernelFn)qs_step_kernel<NP, SPLIT, false, HO, DYN, NZ>;
-}
-
-// The step-kernel instantiation of a launch.  DYN and NZ exist only in the single-warp shape with the grid-wide wait, so
-// `split` and `ho` do not apply to them.
-template <int NP>
-static KernelFn step_kernel(bool split, bool scn, bool ho, bool dyn, bool nz) {
-    if (nz) return dyn ? step_kernel_scn<NP, false, false, true, true>(scn) : step_kernel_scn<NP, false, false, false, true>(scn);
-    if (dyn) return step_kernel_scn<NP, false, false, true, false>(scn);
-    if (split) return ho ? step_kernel_scn<NP, true, true, false, false>(scn) : step_kernel_scn<NP, true, false, false, false>(scn);
-    return ho ? step_kernel_scn<NP, false, true, false, false>(scn) : step_kernel_scn<NP, false, false, false, false>(scn);
+// The numpy dynamics path's step kernels (qs_step_npy.cu): the same shapes, selected by the same rule.
+namespace qs_npy {
+void* step_kernel_npy(int NP, bool split, bool scn, bool ho, bool dyn, bool nz);
 }
 
 struct StepShape {
@@ -438,6 +430,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
                                    p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
     auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
         KernelFn fn = nullptr;
+        if (h->numpy_dyn) return (KernelFn)qs_npy::step_kernel_npy(NP, s.split, scn, ho, k_dyn, k_nz);      // qs_set_numpy_dynamics
         dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
         return fn;
     };
@@ -957,6 +950,13 @@ extern "C" int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, 
     h->init_random = enable ? 1 : 0;
     h->init_vel_max = vel_max;
     h->init_omega_max = omega_max;
+    return QS_OK;
+}
+
+extern "C" int qs_set_numpy_dynamics(QsHandle* h, int enable) {
+    if (!h) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->started) return fail(QS_ERR_INVALID_ARG, "the dynamics path can only be set before the first reset or step");
+    h->numpy_dyn = enable ? 1 : 0;
     return QS_OK;
 }
 

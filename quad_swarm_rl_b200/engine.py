@@ -58,7 +58,8 @@ class QuadSwarmEngine:
                  obst_spawn_area=(8.0, 8.0), use_downwash=False, room_dims=(10., 10., 10.), ep_time=15.0,
                  collision_hitbox_radius=2.0, collision_falloff_radius=4.0, sense_noise='default',
                  approch_goal_metric=0.5, rew_coeff=None, seed=0, device=0, env_id_offset=0,
-                 device_scenario=None, quad_arm=0.0, init_random_state=False, init_vel_max=1.0, init_omega_max=2 * math.pi):
+                 device_scenario=None, quad_arm=0.0, init_random_state=False, init_vel_max=1.0, init_omega_max=2 * math.pi,
+                 use_numba=True):
         if not torch.cuda.is_available():
             raise RuntimeError("QuadSwarmEngine needs a CUDA device (the env step has no CPU path)")
         self.lib = L.load()
@@ -105,6 +106,11 @@ class QuadSwarmEngine:
         self.init_random_state = bool(init_random_state)
         if self.init_random_state:
             L.check(self.lib.qs_set_init_random_state(h, 1, float(init_vel_max), float(init_omega_max)))
+        # QuadrotorEnvMulti(use_numba=False): the physics of the reference's numpy path, whose floor model differs
+        # (QuadrotorDynamics.step1 + floor_interaction, quadrotor_dynamics.py:225-346, 389-457)
+        self.use_numba = bool(use_numba)
+        if not self.use_numba:
+            L.check(self.lib.qs_set_numpy_dynamics(h, 1))
         self.D = self.lib.qs_obs_dim(h)
         self.M = self.lib.qs_num_obstacles(h)
         self.ep_len = self.lib.qs_ep_len(h)

@@ -99,7 +99,7 @@ class _EnvBase:
         self.room_dims = room_dims
         self.quads_view_mode = quads_view_mode
         self.quads_mode = quads_mode
-        self.use_numba = use_numba                          # accepted and ignored: there is one (CUDA) path
+        self.use_numba = use_numba                          # False: the physics of the reference's numpy path (floor model)
         self.use_obstacles = bool(use_obstacles)
         self.use_downwash = bool(use_downwash)
         self.use_replay_buffer = use_replay_buffer
@@ -159,7 +159,7 @@ class _EnvBase:
             ep_time=ep_time, collision_hitbox_radius=collision_hitbox_radius,
             collision_falloff_radius=collision_falloff_radius, sense_noise=sense_noise, rew_coeff=rew_coeff,
             seed=seed, device=device, env_id_offset=env_id_offset, device_scenario=device_scenario, quad_arm=quad_arm,
-            init_random_state=init_random_state,
+            init_random_state=init_random_state, use_numba=bool(use_numba),
             # scenario.approch_goal_metric (o_base.py:16: 1.0 for the goal-sharing obstacle scenarios, else 0.5); with the
             # host-side `mix` over obstacle scenarios the value of o_random is used for every episode
             approch_goal_metric=1.0 if quads_mode in ('o_static_same_goal', 'o_dynamic_same_goal', 'o_swap_goals',
@@ -477,7 +477,7 @@ class QuadrotorEnvMultiBatched(_EnvBase):
                  obst_spawn_area=(8.0, 8.0), use_downwash=False, quads_mode='static_same_goal',
                  room_dims=(10., 10., 10.), sense_noise='default', device=0, seed=None, env_id_offset=0,
                  device_scenarios=True, dynamics_params='Crazyflie', dynamics_randomize_every=None, dynamics_change=None,
-                 dyn_sampler_1=None, init_random_state=False):
+                 dyn_sampler_1=None, init_random_state=False, use_numba=True):
         # device-side generators (no host work per episode or per tick): o_random with obstacles, the goal-formation
         # family and mix without; every other mode uses host tables
         dev_scn = None
@@ -487,7 +487,7 @@ class QuadrotorEnvMultiBatched(_EnvBase):
             dev_scn = quads_mode
         super().__init__(num_envs, num_agents, ep_time, rew_coeff, obs_repr, neighbor_visible_num, neighbor_obs_type,
                          collision_hitbox_radius, collision_falloff_radius, use_obstacles, obst_density, obst_size,
-                         obst_spawn_area, use_downwash, True, quads_mode, room_dims, False, ['topdown'], False,
+                         obst_spawn_area, use_downwash, use_numba, quads_mode, room_dims, False, ['topdown'], False,
                          dynamics_params, True, True, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise,
                          init_random_state, device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn)
         self.num_agents = num_envs * num_agents

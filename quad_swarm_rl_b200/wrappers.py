@@ -131,7 +131,9 @@ def make_quadrotor_env_multi_batched(cfg, num_envs, env_id_offset=0, stats_every
         obst_size=cfg.quads_obst_size,
         obst_spawn_area=cfg.quads_obst_spawn_area, use_downwash=cfg.quads_use_downwash, quads_mode=cfg.quads_mode,
         room_dims=cfg.quads_room_dims, device=getattr(cfg, 'quads_device', 0), seed=getattr(cfg, 'seed', None),
-        env_id_offset=env_id_offset)
+        env_id_offset=env_id_offset,
+        # --quads_use_numba (quadrotor_params.py:88, default False); an object without the attribute keeps the njit path
+        use_numba=getattr(cfg, 'quads_use_numba', True))
     # quad_utils.py:67-70: domain randomisation of the pillar field (per fresh episode, on the device)
     if cfg.quads_use_obstacles and getattr(cfg, 'quads_domain_random', False) and env.device_scenario is not None:
         dens = [cfg.quads_obst_density]
