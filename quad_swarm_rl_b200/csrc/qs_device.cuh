@@ -37,7 +37,7 @@ constexpr float MOTOR_TAU_UP = 0.13333244445037035f, MOTOR_TAU_DOWN = 0.13333244
 constexpr float OMEGA_MAX = 40.0f;
 constexpr float FLOOR_MU = 0.6f;
 // QS_NUMPY_DYNAMICS = 1 (set by qs_step_npy.cu only): the floor model of the reference's numpy path (use_numba=False;
-// QuadrotorDynamics.floor_interaction, quadrotor_dynamics.py:389-457) in dynamics_substep() / dynamics_substep_dyn().
+// QuadrotorDynamics.floor_interaction, quadrotor_dynamics.py:389-457) in physics_substep().
 #ifndef QS_NUMPY_DYNAMICS
 #define QS_NUMPY_DYNAMICS 0
 #endif
@@ -272,29 +272,113 @@ __device__ __forceinline__ void friction_dir_numpy(float vx, float h2, float& ca
 }
 #endif
 
+// ---- per-drone physical constants (SURVEY 8f-4: dynamics randomisation, non-Crazyflie models, rotor drag) ----
+// Row layout = QS_DYN_* of include/quadswarm.h = quad_models.DYN_FIELDS: what QuadrotorDynamics.update_model derives
+// (quadrotor_dynamics.py:104-166).  Kernels instantiated with DYN = false keep the compile-time Crazyflie constants above.
+struct Phys {
+    float mass, inv_mass, ixx, iyy, izz, inv_ixx, inv_iyy, inv_izz;
+    float thrust_max[4], torque_max[4];
+    float px[4], py[4], pz[4];
+    float tau_up, tau_down, linearity, ou_sigma, c_drag, c_roll, vel_damp, omega_quadratic, arm;
+};
+
+__device__ __forceinline__ void load_phys(const float4* rows, long long a, Phys& ph) {
+    const float4* r = rows + a * (QS_DYN_ROW / 4);
+    const float4 q0 = QS_LD(r + 0), q1 = QS_LD(r + 1), q2 = QS_LD(r + 2), q3 = QS_LD(r + 3), q4 = QS_LD(r + 4), q5 = QS_LD(r + 5),
+                 q6 = QS_LD(r + 6), q7 = QS_LD(r + 7), q8 = QS_LD(r + 8), q9 = QS_LD(r + 9);
+    ph.mass = q0.x; ph.inv_mass = q0.y; ph.ixx = q0.z; ph.iyy = q0.w;
+    ph.izz = q1.x; ph.inv_ixx = q1.y; ph.inv_iyy = q1.z; ph.inv_izz = q1.w;
+    ph.thrust_max[0] = q2.x; ph.thrust_max[1] = q2.y; ph.thrust_max[2] = q2.z; ph.thrust_max[3] = q2.w;
+    ph.torque_max[0] = q3.x; ph.torque_max[1] = q3.y; ph.torque_max[2] = q3.z; ph.torque_max[3] = q3.w;
+    ph.px[0] = q4.x; ph.py[0] = q4.y; ph.px[1] = q4.z; ph.py[1] = q4.w;
+    ph.px[2] = q5.x; ph.py[2] = q5.y; ph.px[3] = q5.z; ph.py[3] = q5.w;
+    ph.pz[0] = q6.x; ph.pz[1] = q6.y; ph.pz[2] = q6.z; ph.pz[3] = q6.w;
+    ph.tau_up = q7.x; ph.tau_down = q7.y; ph.linearity = q7.z; ph.ou_sigma = q7.w;
+    ph.c_drag = q8.x; ph.c_roll = q8.y; ph.vel_damp = q8.z; ph.omega_quadratic = q8.w;
+    ph.arm = q9.x;
+}
+
 // One 5 ms physics sub-step of the njit path: step1_numba, quadrotor_dynamics.py:348-383
 // (calculate_torque_integrate_rotations_and_update_omega :497-566, room clip :360-367,
 //  floor_interaction_numba :569-639, compute_velocity_and_acceleration :642-649).
 // `cmd` is the RawControl output in [0,1]; the OU state s.ou is the thrust noise of this control step.
+// DYN = false: the compile-time Crazyflie constants; `ph` is not read.  DYN = true: the per-drone constants `ph` — general
+// motor asymmetry / linearity / propeller positions / damping — plus the rotor-drag and rolling-moment term that only the
+// reference's numpy path has (step1, quadrotor_dynamics.py:256-289; all shipped models have C_drag = C_roll = 0).
+// The Crazyflie arms are not the general formulas with constant values: IEEE arithmetic does not fold terms such as
+// (1 - linearity) cd^2 or 1 - clamp(0 ox^2) away, so those would change the default kernels' arithmetic.
 // QS_NUMPY_DYNAMICS: the floor model of the numpy path instead (floor_interaction, :389-457).
-template <bool FMA_FRICTION = false>
-__device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], bool do_svd, const StepParams& p,
-                                                 const RngKey& key, int i, int sub) {
-    // motor lag on sqrt(thrust) + OU thrust noise (:504-517); linearity = 1 so thrust = thrust_max * cmds_damp
+template <bool DYN, bool FMA_FRICTION>
+__device__ __forceinline__ void physics_substep(Agent& s, const float cmd[4], bool do_svd, const StepParams& p,
+                                                const RngKey& key, int i, int sub, const Phys& ph) {
+    static_assert(!(DYN && FMA_FRICTION), "the fused friction form is written with the Crazyflie mass");
     float thr[4];
+    float tq0, tq1, tq2, thrust_z;
+    float drag_fx = 0.f, drag_fy = 0.f, drag_fz = 0.f;      // body-frame rotor drag (DYN)
+    if constexpr (DYN) {
+        tq0 = 0.f; tq1 = 0.f; tq2 = 0.f; thrust_z = 0.f;
 #pragma unroll
-    for (int m = 0; m < 4; ++m) {
-        const float c = cmd[m];                       // already in [0,1]; the second np.clip (:504) is a no-op
-        const float tau = fminf((c < s.cd[m]) ? MOTOR_TAU_DOWN : MOTOR_TAU_UP, 1.f);
-        s.rd[m] = tau * (fsqrt(c) - s.rd[m]) + s.rd[m];
-        s.cd[m] = clampf(s.rd[m] * s.rd[m] + c * s.ou[m], 0.f, 1.f);
-        thr[m] = THRUST_MAX * s.cd[m];
+        for (int m = 0; m < 4; ++m) {
+            const float c = cmd[m];
+            const float tau = fminf((c < s.cd[m]) ? ph.tau_down : ph.tau_up, 1.f);
+            s.rd[m] = tau * (fsqrt(c) - s.rd[m]) + s.rd[m];
+            s.cd[m] = clampf(s.rd[m] * s.rd[m] + c * s.ou[m], 0.f, 1.f);
+            thr[m] = ph.thrust_max[m] * ((1.f - ph.linearity) * s.cd[m] * s.cd[m] + ph.linearity * s.cd[m]);   // numba_utils.py:58-60
+            // prop_crossproducts = cross(prop_pos, z) = (py, -px, 0) (quadrotor_dynamics.py:141); prop_ccw = (-1, 1, -1, 1)
+            tq0 += ph.py[m] * thr[m];
+            tq1 += -ph.px[m] * thr[m];
+            tq2 += ((m & 1) ? 1.f : -1.f) * ph.torque_max[m] * s.cd[m];
+            thrust_z += thr[m];
+        }
+        if (ph.c_drag != 0.f || ph.c_roll != 0.f) {
+            // body-frame velocity of every rotor hub, projected on the rotor plane
+            const float vbx = s.R[0] * s.vel[0] + s.R[3] * s.vel[1] + s.R[6] * s.vel[2];
+            const float vby = s.R[1] * s.vel[0] + s.R[4] * s.vel[1] + s.R[7] * s.vel[2];
+            const float vbz = s.R[2] * s.vel[0] + s.R[5] * s.vel[1] + s.R[8] * s.vel[2];
+            float tx = 0.f, ty = 0.f, tz = 0.f;
+#pragma unroll
+            for (int m = 0; m < 4; ++m) {
+                const float vrx = vbx + (s.om[1] * ph.pz[m] - s.om[2] * ph.py[m]);       // v + omega x prop_pos
+                const float vry = vby + (s.om[2] * ph.px[m] - s.om[0] * ph.pz[m]);
+                const float sq = sqrtf(s.cd[m]);
+                const float fix = -ph.c_drag * sq * vrx, fiy = -ph.c_drag * sq * vry;     // drag force of rotor m (z component 0)
+                drag_fx += fix; drag_fy += fiy;
+                // torque = f_i x prop_pos, plus the rolling moment -C_roll ccw sqrt(c) v_rotor
+                tx += fiy * ph.pz[m]; ty += -fix * ph.pz[m]; tz += fix * ph.py[m] - fiy * ph.px[m];
+                const float ccw = (m & 1) ? 1.f : -1.f;
+                tx += -ph.c_roll * ccw * sq * vrx; ty += -ph.c_roll * ccw * sq * vry;
+            }
+            const float dt2 = 2.f * SIM_DT;
+            const float vel_norm = norm3(vbx, vby, vbz);
+            const float rdf = sqrtf(drag_fx * drag_fx + drag_fy * drag_fy);
+            if (rdf > EPS_DYN) {
+                const float sc = fminf(rdf, vel_norm * ph.mass / dt2) / rdf;
+                drag_fx *= sc; drag_fy *= sc;
+            }
+            const float rvt = sqrtf(tx * tx + ty * ty + tz * tz);
+            if (rvt > EPS_DYN) {
+                const float lim = norm3(s.om[0] * ph.ixx, s.om[1] * ph.iyy, s.om[2] * ph.izz) / dt2;
+                const float sc = fminf(rvt, lim) / rvt;
+                tx *= sc; ty *= sc; tz *= sc;
+            }
+            tq0 += tx; tq1 += ty; tq2 += tz;
+        }
+    } else {
+        // motor lag on sqrt(thrust) + OU thrust noise (:504-517); linearity = 1 so thrust = thrust_max * cmds_damp
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+            const float c = cmd[m];                       // already in [0,1]; the second np.clip (:504) is a no-op
+            const float tau = fminf((c < s.cd[m]) ? MOTOR_TAU_DOWN : MOTOR_TAU_UP, 1.f);
+            s.rd[m] = tau * (fsqrt(c) - s.rd[m]) + s.rd[m];
+            s.cd[m] = clampf(s.rd[m] * s.rd[m] + c * s.ou[m], 0.f, 1.f);
+            thr[m] = THRUST_MAX * s.cd[m];
+        }
+        // torques: prop_crossproducts x thrust, plus rotor reaction torque about z (:520-526); rotor drag is zero (:529)
+        tq0 = PROP_ARM_XY * ((thr[2] + thr[3]) - (thr[0] + thr[1]));
+        tq1 = PROP_ARM_XY * ((thr[1] + thr[2]) - (thr[0] + thr[3]));
+        tq2 = TORQUE_MAX * ((s.cd[1] + s.cd[3]) - (s.cd[0] + s.cd[2]));
+        thrust_z = (thr[0] + thr[1]) + (thr[2] + thr[3]);
     }
-    // torques: prop_crossproducts x thrust, plus rotor reaction torque about z (:520-526); rotor drag is zero (:529)
-    const float tq0 = PROP_ARM_XY * ((thr[2] + thr[3]) - (thr[0] + thr[1]));
-    const float tq1 = PROP_ARM_XY * ((thr[1] + thr[2]) - (thr[0] + thr[3]));
-    const float tq2 = TORQUE_MAX * ((s.cd[1] + s.cd[3]) - (s.cd[0] + s.cd[2]));
-    const float thrust_z = (thr[0] + thr[1]) + (thr[2] + thr[3]);
 
     // Rodrigues rotation by the world-frame angular velocity w (:537-544):
     //   R <- (I + sin(t) K + (1 - cos(t)) K^2) R,  K = [w]x / |w|,  t = |w| dt
@@ -327,8 +411,17 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
         for (int k = 0; k < 9; ++k) s.R[k] = m.m[k];
     }
 
-    // Euler step of the body rates with gyroscopic term (:555-560); quadratic damping is zero
-    {
+    // Euler step of the body rates with gyroscopic term (:555-560); the Crazyflie's quadratic damping is zero
+    if constexpr (DYN) {
+        const float ox = s.om[0], oy = s.om[1], oz = s.om[2];
+        const float ix = ph.ixx * ox, iy = ph.iyy * oy, iz = ph.izz * oz;
+        const float cxx = oz * iy - oy * iz, cyy = ox * iz - oz * ix, czz = oy * ix - ox * iy;
+        const float dx = 1.f - clampf(ph.omega_quadratic * ox * ox, 0.f, 1.f), dy = 1.f - clampf(ph.omega_quadratic * oy * oy, 0.f, 1.f),
+                    dz = 1.f - clampf(ph.omega_quadratic * oz * oz, 0.f, 1.f);
+        s.om[0] = clampf(ox + dx * SIM_DT * (ph.inv_ixx * (cxx + tq0)), -OMEGA_MAX, OMEGA_MAX);
+        s.om[1] = clampf(oy + dy * SIM_DT * (ph.inv_iyy * (cyy + tq1)), -OMEGA_MAX, OMEGA_MAX);
+        s.om[2] = clampf(oz + dz * SIM_DT * (ph.inv_izz * (czz + tq2)), -OMEGA_MAX, OMEGA_MAX);
+    } else {
         const float ox = s.om[0], oy = s.om[1], oz = s.om[2];
         const float ix = IXX * ox, iy = IYY * oy, iz = IZZ * oz;
         const float cxx = oz * iy - oy * iz;          // cross(-omega, I omega)
@@ -347,22 +440,33 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
     if (px != s.pos[0] || py != s.pos[1]) fl |= QS_FLAG_CRASHED_WALL;
     if (pz > s.pos[2]) fl |= QS_FLAG_CRASHED_CEILING;
 
-    // floor contact / friction, threshold = arm (:569-639).  Numpy path: threshold 0.05 (:75), exact at-rest test (:406),
-    // friction along the velocity (:419-422), re-drawn landing yaw (:434-437)
+    // force in the world frame: R (thrust + rotor drag)
+    const float r22 = s.R[8];
+    float fx, fy, fz;
+    if constexpr (DYN) {
+        fx = s.R[0] * drag_fx + s.R[1] * drag_fy + s.R[2] * (thrust_z + drag_fz);
+        fy = s.R[3] * drag_fx + s.R[4] * drag_fy + s.R[5] * (thrust_z + drag_fz);
+        fz = s.R[6] * drag_fx + s.R[7] * drag_fy + s.R[8] * (thrust_z + drag_fz);
+    } else {
+        fx = s.R[2] * thrust_z; fy = s.R[5] * thrust_z; fz = r22 * thrust_z;
+    }
+    const float mass = DYN ? ph.mass : MASS, inv_mass = DYN ? ph.inv_mass : INV_MASS;
+    const float keep = DYN ? 1.f - ph.vel_damp : 1.f;      // the Crazyflie's vel_damp is zero, and 1.f * v is exact
+
+    // floor contact / friction, threshold = the arm (:569-639, :378).  Numpy path: threshold 0.05 (:75), exact at-rest
+    // test (:406), friction along the velocity (:419-422), re-drawn landing yaw (:434-437)
 #if QS_NUMPY_DYNAMICS
-    constexpr float floor_z = FLOOR_THRESHOLD_NP;
+    const float floor_z = FLOOR_THRESHOLD_NP;
 #else
-    constexpr float floor_z = ARM;
+    const float floor_z = DYN ? ph.arm : ARM;
 #endif
-    float fx = s.R[2] * thrust_z, fy = s.R[5] * thrust_z;
-    const float r22 = s.R[8], fz = r22 * thrust_z;
     if (s.pos[2] <= floor_z) {
         s.pos[2] = floor_z;
         if (fl & QS_FLAG_ON_FLOOR) {
             yaw_only(s.R);
             // FMA_FRICTION: MASS * GRAV - fz with one rounding, written out.  The compiler fused it in these kernels before
             // their register cap and no longer does; the other kernels keep the expression (and the compiler's choice) as it was.
-            const float fric = FLOOR_MU * (FMA_FRICTION ? __fmaf_rn(-r22, thrust_z, MASS * GRAV) : MASS * GRAV - fz);
+            const float fric = FLOOR_MU * (FMA_FRICTION ? __fmaf_rn(-r22, thrust_z, MASS * GRAV) : mass * GRAV - fz);
 #if QS_NUMPY_DYNAMICS
             if (s.vel[0] == 0.f && s.vel[1] == 0.f && s.vel[2] == 0.f) {       // :406
 #else
@@ -411,213 +515,30 @@ __device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], b
             for (int m = 0; m < 4; ++m) { s.rd[m] = 0.f; s.cd[m] = 0.f; }
         }
         // the force was taken with the pre-flattening rotation (:576), as here
-        s.vel[0] += SIM_DT * (INV_MASS * fx);
-        s.vel[1] += SIM_DT * (INV_MASS * fy);
-        s.vel[2] += SIM_DT * fmaxf(0.f, -GRAV + INV_MASS * fz);
+        s.vel[0] = keep * s.vel[0] + SIM_DT * (inv_mass * fx);
+        s.vel[1] = keep * s.vel[1] + SIM_DT * (inv_mass * fy);
+        s.vel[2] = keep * s.vel[2] + SIM_DT * fmaxf(0.f, -GRAV + inv_mass * fz);
     } else {
         fl &= ~QS_FLAG_ON_FLOOR;
-        s.vel[0] += SIM_DT * (INV_MASS * fx);
-        s.vel[1] += SIM_DT * (INV_MASS * fy);
-        s.vel[2] += SIM_DT * (-GRAV + INV_MASS * fz);
+        s.vel[0] = keep * s.vel[0] + SIM_DT * (inv_mass * fx);
+        s.vel[1] = keep * s.vel[1] + SIM_DT * (inv_mass * fy);
+        s.vel[2] = keep * s.vel[2] + SIM_DT * (-GRAV + inv_mass * fz);
     }
     s.flags = fl;
-    // velocity used the NEW acceleration (:645); vel_damp = 0.  The accelerometer reading (:648) is never observed.
+    // velocity used the NEW acceleration (:645).  The accelerometer reading (:648) is never observed.
 }
 
-// ---- per-drone physical constants (SURVEY 8f-4: dynamics randomisation, non-Crazyflie models, rotor drag) ----
-// Row layout = QS_DYN_* of include/quadswarm.h = quad_models.DYN_FIELDS: what QuadrotorDynamics.update_model derives
-// (quadrotor_dynamics.py:104-166).  Kernels instantiated with DYN = false keep the compile-time Crazyflie constants above.
-struct Phys {
-    float mass, inv_mass, ixx, iyy, izz, inv_ixx, inv_iyy, inv_izz;
-    float thrust_max[4], torque_max[4];
-    float px[4], py[4], pz[4];
-    float tau_up, tau_down, linearity, ou_sigma, c_drag, c_roll, vel_damp, omega_quadratic, arm;
-};
-
-__device__ __forceinline__ void load_phys(const float4* rows, long long a, Phys& ph) {
-    const float4* r = rows + a * (QS_DYN_ROW / 4);
-    const float4 q0 = QS_LD(r + 0), q1 = QS_LD(r + 1), q2 = QS_LD(r + 2), q3 = QS_LD(r + 3), q4 = QS_LD(r + 4), q5 = QS_LD(r + 5),
-                 q6 = QS_LD(r + 6), q7 = QS_LD(r + 7), q8 = QS_LD(r + 8), q9 = QS_LD(r + 9);
-    ph.mass = q0.x; ph.inv_mass = q0.y; ph.ixx = q0.z; ph.iyy = q0.w;
-    ph.izz = q1.x; ph.inv_ixx = q1.y; ph.inv_iyy = q1.z; ph.inv_izz = q1.w;
-    ph.thrust_max[0] = q2.x; ph.thrust_max[1] = q2.y; ph.thrust_max[2] = q2.z; ph.thrust_max[3] = q2.w;
-    ph.torque_max[0] = q3.x; ph.torque_max[1] = q3.y; ph.torque_max[2] = q3.z; ph.torque_max[3] = q3.w;
-    ph.px[0] = q4.x; ph.py[0] = q4.y; ph.px[1] = q4.z; ph.py[1] = q4.w;
-    ph.px[2] = q5.x; ph.py[2] = q5.y; ph.px[3] = q5.z; ph.py[3] = q5.w;
-    ph.pz[0] = q6.x; ph.pz[1] = q6.y; ph.pz[2] = q6.z; ph.pz[3] = q6.w;
-    ph.tau_up = q7.x; ph.tau_down = q7.y; ph.linearity = q7.z; ph.ou_sigma = q7.w;
-    ph.c_drag = q8.x; ph.c_roll = q8.y; ph.vel_damp = q8.z; ph.omega_quadratic = q8.w;
-    ph.arm = q9.x;
+// The default step kernels: Crazyflie constants, inlined into the kernel.
+template <bool FMA_FRICTION = false>
+__device__ __forceinline__ void dynamics_substep(Agent& s, const float cmd[4], bool do_svd, const StepParams& p,
+                                                 const RngKey& key, int i, int sub) {
+    physics_substep<false, FMA_FRICTION>(s, cmd, do_svd, p, key, i, sub, Phys{});
 }
 
-// One 5 ms physics sub-step with per-drone constants: the njit path as in dynamics_substep() above — general motor
-// asymmetry / linearity / propeller positions / damping — plus the rotor-drag and rolling-moment term that only the
-// reference's numpy path has (step1, quadrotor_dynamics.py:256-289; all shipped models have C_drag = C_roll = 0).
-// QS_NUMPY_DYNAMICS: the numpy path's floor model, as in dynamics_substep().
+// The DYN step kernels: per-drone constants, out of line.
 __device__ __noinline__ void dynamics_substep_dyn(Agent& s, const float cmd[4], bool do_svd, const StepParams& p, const RngKey& key,
                                                   int i, int sub, const Phys& ph) {
-    float thr[4];
-    float tq0 = 0.f, tq1 = 0.f, tq2 = 0.f, thrust_z = 0.f;
-#pragma unroll
-    for (int m = 0; m < 4; ++m) {
-        const float c = cmd[m];
-        const float tau = fminf((c < s.cd[m]) ? ph.tau_down : ph.tau_up, 1.f);
-        s.rd[m] = tau * (fsqrt(c) - s.rd[m]) + s.rd[m];
-        s.cd[m] = clampf(s.rd[m] * s.rd[m] + c * s.ou[m], 0.f, 1.f);
-        thr[m] = ph.thrust_max[m] * ((1.f - ph.linearity) * s.cd[m] * s.cd[m] + ph.linearity * s.cd[m]);   // numba_utils.py:58-60
-        // prop_crossproducts = cross(prop_pos, z) = (py, -px, 0) (quadrotor_dynamics.py:141); prop_ccw = (-1, 1, -1, 1)
-        tq0 += ph.py[m] * thr[m];
-        tq1 += -ph.px[m] * thr[m];
-        tq2 += ((m & 1) ? 1.f : -1.f) * ph.torque_max[m] * s.cd[m];
-        thrust_z += thr[m];
-    }
-    float drag_fx = 0.f, drag_fy = 0.f, drag_fz = 0.f;
-    if (ph.c_drag != 0.f || ph.c_roll != 0.f) {
-        // body-frame velocity of every rotor hub, projected on the rotor plane
-        const float vbx = s.R[0] * s.vel[0] + s.R[3] * s.vel[1] + s.R[6] * s.vel[2];
-        const float vby = s.R[1] * s.vel[0] + s.R[4] * s.vel[1] + s.R[7] * s.vel[2];
-        const float vbz = s.R[2] * s.vel[0] + s.R[5] * s.vel[1] + s.R[8] * s.vel[2];
-        float tx = 0.f, ty = 0.f, tz = 0.f;
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-            const float vrx = vbx + (s.om[1] * ph.pz[m] - s.om[2] * ph.py[m]);       // v + omega x prop_pos
-            const float vry = vby + (s.om[2] * ph.px[m] - s.om[0] * ph.pz[m]);
-            const float sq = sqrtf(s.cd[m]);
-            const float fix = -ph.c_drag * sq * vrx, fiy = -ph.c_drag * sq * vry;     // drag force of rotor m (z component 0)
-            drag_fx += fix; drag_fy += fiy;
-            // torque = f_i x prop_pos, plus the rolling moment -C_roll ccw sqrt(c) v_rotor
-            tx += fiy * ph.pz[m]; ty += -fix * ph.pz[m]; tz += fix * ph.py[m] - fiy * ph.px[m];
-            const float ccw = (m & 1) ? 1.f : -1.f;
-            tx += -ph.c_roll * ccw * sq * vrx; ty += -ph.c_roll * ccw * sq * vry;
-        }
-        const float dt2 = 2.f * SIM_DT;
-        const float vel_norm = norm3(vbx, vby, vbz);
-        const float rdf = sqrtf(drag_fx * drag_fx + drag_fy * drag_fy);
-        if (rdf > EPS_DYN) {
-            const float sc = fminf(rdf, vel_norm * ph.mass / dt2) / rdf;
-            drag_fx *= sc; drag_fy *= sc;
-        }
-        const float rvt = sqrtf(tx * tx + ty * ty + tz * tz);
-        if (rvt > EPS_DYN) {
-            const float lim = norm3(s.om[0] * ph.ixx, s.om[1] * ph.iyy, s.om[2] * ph.izz) / dt2;
-            const float sc = fminf(rvt, lim) / rvt;
-            tx *= sc; ty *= sc; tz *= sc;
-        }
-        tq0 += tx; tq1 += ty; tq2 += tz;
-    }
-
-    {   // Rodrigues update, as in dynamics_substep()
-        const float wx = s.R[0] * s.om[0] + s.R[1] * s.om[1] + s.R[2] * s.om[2];
-        const float wy = s.R[3] * s.om[0] + s.R[4] * s.om[1] + s.R[5] * s.om[2];
-        const float wz = s.R[6] * s.om[0] + s.R[7] * s.om[1] + s.R[8] * s.om[2];
-        const float w2 = wx * wx + wy * wy + wz * wz;
-        const float t2 = w2 * (SIM_DT * SIM_DT);
-        const float ca = SIM_DT * (1.f + t2 * (-1.f / 6.f + t2 * (1.f / 120.f + t2 * (-1.f / 5040.f))));
-        const float cb = (SIM_DT * SIM_DT) * (0.5f + t2 * (-1.f / 24.f + t2 * (1.f / 720.f + t2 * (-1.f / 40320.f))));
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float vx = s.R[c], vy = s.R[3 + c], vz = s.R[6 + c];
-            const float wd = wx * vx + wy * vy + wz * vz;
-            s.R[c] = vx + ca * (wy * vz - wz * vy) + cb * (wx * wd - vx * w2);
-            s.R[3 + c] = vy + ca * (wz * vx - wx * vz) + cb * (wy * wd - vy * w2);
-            s.R[6 + c] = vz + ca * (wx * vy - wy * vx) + cb * (wz * wd - vz * w2);
-        }
-    }
-    if (do_svd) {
-        M3 m;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) m.m[k] = s.R[k];
-        m = orthonormalize(m);
-#pragma unroll
-        for (int k = 0; k < 9; ++k) s.R[k] = m.m[k];
-    }
-    {   // body rates (:555-560) with quadratic damping
-        const float ox = s.om[0], oy = s.om[1], oz = s.om[2];
-        const float ix = ph.ixx * ox, iy = ph.iyy * oy, iz = ph.izz * oz;
-        const float cxx = oz * iy - oy * iz, cyy = ox * iz - oz * ix, czz = oy * ix - ox * iy;
-        const float dx = 1.f - clampf(ph.omega_quadratic * ox * ox, 0.f, 1.f), dy = 1.f - clampf(ph.omega_quadratic * oy * oy, 0.f, 1.f),
-                    dz = 1.f - clampf(ph.omega_quadratic * oz * oz, 0.f, 1.f);
-        s.om[0] = clampf(ox + dx * SIM_DT * (ph.inv_ixx * (cxx + tq0)), -OMEGA_MAX, OMEGA_MAX);
-        s.om[1] = clampf(oy + dy * SIM_DT * (ph.inv_iyy * (cyy + tq1)), -OMEGA_MAX, OMEGA_MAX);
-        s.om[2] = clampf(oz + dz * SIM_DT * (ph.inv_izz * (czz + tq2)), -OMEGA_MAX, OMEGA_MAX);
-    }
-    const float px = s.pos[0] + SIM_DT * s.vel[0], py = s.pos[1] + SIM_DT * s.vel[1], pz = s.pos[2] + SIM_DT * s.vel[2];
-    s.pos[0] = clampf(px, p.room_lo[0], p.room_hi[0]);
-    s.pos[1] = clampf(py, p.room_lo[1], p.room_hi[1]);
-    s.pos[2] = clampf(pz, p.room_lo[2], p.room_hi[2]);
-    uint32_t fl = s.flags & ~(QS_FLAG_CRASHED_WALL | QS_FLAG_CRASHED_CEILING | QS_FLAG_CRASHED_FLOOR);
-    if (px != s.pos[0] || py != s.pos[1]) fl |= QS_FLAG_CRASHED_WALL;
-    if (pz > s.pos[2]) fl |= QS_FLAG_CRASHED_CEILING;
-
-    // force in the world frame: R (thrust + rotor drag), floor contact with threshold = this drone's arm (:378), or 0.05
-    float fx = s.R[0] * drag_fx + s.R[1] * drag_fy + s.R[2] * (thrust_z + drag_fz);
-    float fy = s.R[3] * drag_fx + s.R[4] * drag_fy + s.R[5] * (thrust_z + drag_fz);
-    const float fz = s.R[6] * drag_fx + s.R[7] * drag_fy + s.R[8] * (thrust_z + drag_fz);
-    const float keep = 1.f - ph.vel_damp;
-#if QS_NUMPY_DYNAMICS
-    const float floor_z = FLOOR_THRESHOLD_NP;
-#else
-    const float floor_z = ph.arm;
-#endif
-    if (s.pos[2] <= floor_z) {
-        s.pos[2] = floor_z;
-        if (fl & QS_FLAG_ON_FLOOR) {
-            yaw_only(s.R);
-            const float fric = FLOOR_MU * (ph.mass * GRAV - fz);
-#if QS_NUMPY_DYNAMICS
-            if (s.vel[0] == 0.f && s.vel[1] == 0.f && s.vel[2] == 0.f) {
-#else
-            const float v2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1] + s.vel[2] * s.vel[2];
-            if (v2 < EPS_DYN * EPS_DYN) {
-#endif
-                const float fm = fsqrt(fx * fx + fy * fy);
-                const float mag = fmaxf(fm - fric, 0.f);
-                if (fm > 0.f) {
-                    const float sc = mag * frcp(fm);
-                    fx *= sc; fy *= sc;
-                } else {
-                    fx = mag; fy = 0.f;
-                }
-            } else {
-                const float h2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1];
-                float ca = 1.f, sa = 0.f;
-                if (h2 > 0.f) {
-                    const float inv = frsqrt(h2);
-                    ca = s.vel[0] * inv; sa = s.vel[1] * inv;
-                }
-#if QS_NUMPY_DYNAMICS
-                friction_dir_numpy(s.vel[0], h2, ca, sa);
-#endif
-                fx -= ca * fric; fy -= sa * fric;
-            }
-        } else {
-            fl |= QS_FLAG_ON_FLOOR | QS_FLAG_CRASHED_FLOOR;
-            s.vel[0] = s.vel[1] = s.vel[2] = 0.f;
-            s.om[0] = s.om[1] = s.om[2] = 0.f;
-            if (s.R[8] < 0.f) {
-#if QS_NUMPY_DYNAMICS
-                const float2 cs = floor_yaw_numpy(key, i, sub, s.pos[0], s.pos[1]);
-#else
-                const float2 cs = floor_random_yaw(key, i, sub);
-#endif
-                s.R[0] = cs.x; s.R[1] = -cs.y; s.R[2] = 0.f; s.R[3] = cs.y; s.R[4] = cs.x; s.R[5] = 0.f;
-                s.R[6] = 0.f; s.R[7] = 0.f; s.R[8] = 1.f;
-            } else {
-                yaw_only(s.R);
-            }
-#pragma unroll
-            for (int m = 0; m < 4; ++m) { s.rd[m] = 0.f; s.cd[m] = 0.f; }
-        }
-        s.vel[0] = keep * s.vel[0] + SIM_DT * (ph.inv_mass * fx);
-        s.vel[1] = keep * s.vel[1] + SIM_DT * (ph.inv_mass * fy);
-        s.vel[2] = keep * s.vel[2] + SIM_DT * fmaxf(0.f, -GRAV + ph.inv_mass * fz);
-    } else {
-        fl &= ~QS_FLAG_ON_FLOOR;
-        s.vel[0] = keep * s.vel[0] + SIM_DT * (ph.inv_mass * fx);
-        s.vel[1] = keep * s.vel[1] + SIM_DT * (ph.inv_mass * fy);
-        s.vel[2] = keep * s.vel[2] + SIM_DT * (-GRAV + ph.inv_mass * fz);
-    }
-    s.flags = fl;
+    physics_substep<true, false>(s, cmd, do_svd, p, key, i, sub, ph);
 }
 
 // Observed rotation quat2R(rot2quat(R) x qt) (sensor_noise.py:34-63,205-210; quad_utils.py:133-159); qt is the
