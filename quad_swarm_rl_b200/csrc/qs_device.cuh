@@ -217,6 +217,23 @@ __device__ __forceinline__ void store_agent(const DevState& st, long long a, con
     if (store_goal) p[SL_GOAL * st.a_pad] = make_float4(s.goal[0], s.goal[1], s.goal[2], 0.f);
 }
 
+// state of a lane without a drone: at rest, level, and far from every other lane (it takes part in the shuffles of its warp)
+__device__ __forceinline__ void idle_agent(Agent& s, int i) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { s.pos[k] = 1e9f + 1e6f * i; s.vel[k] = 0.f; s.om[k] = 0.f; s.goal[k] = 0.f; }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) s.R[k] = (k % 4 == 0) ? 1.f : 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { s.rd[k] = 0.f; s.cd[k] = 0.f; s.ou[k] = 0.f; s.ring[k] = 0.f; }
+    s.flags = 0u; s.prev_col = 0u;
+}
+
+// new velocity and body-rate increment of a contact response (obstacle, wall, ceiling)
+__device__ __forceinline__ void apply_kick(Agent& s, const KickVO& o) {
+    s.vel[0] = o.vel.x; s.vel[1] = o.vel.y; s.vel[2] = o.vel.z;
+    s.om[0] += o.dom.x; s.om[1] += o.dom.y; s.om[2] += o.dom.z;
+}
+
 // R -> pure yaw (quadrotor_dynamics.py:579-581, :614-621): theta = atan2(R10, R00 + eps), then (cos, sin) of it.
 // cos(atan2(y, x)) = x / hypot, so no trigonometry is needed; atan2(0, 0) = 0 gives the identity.
 __device__ __forceinline__ void yaw_only(float R[9]) {
@@ -590,6 +607,16 @@ __device__ __noinline__ Noise9 sensor_noise(RngKey key, uint32_t site, int i) {
     o.v[0] = VEL_NOISE_STD * n[3]; o.v[1] = VEL_NOISE_STD * n[4]; o.v[2] = VEL_NOISE_STD * n[5];
     o.w[0] = GYRO_NOISE_STD * n[6]; o.w[1] = GYRO_NOISE_STD * n[7]; o.w[2] = GYRO_NOISE_STD * n[8];
     return o;
+}
+
+// the 'default' set's first sensor-noise draw of a step, scaled from the hot normals (SITE_HOT); zero with sensor noise off
+__device__ __forceinline__ Noise9 default_noise(const HotNormals& hn, int sense_noise) {
+    const float on = sense_noise ? 1.f : 0.f;
+    Noise9 nz;
+    nz.p[0] = on * POS_NOISE_STD * hn.sn[0]; nz.p[1] = on * POS_NOISE_STD * hn.sn[1]; nz.p[2] = on * POS_NOISE_STD * hn.sn[2];
+    nz.v[0] = on * VEL_NOISE_STD * hn.sn[3]; nz.v[1] = on * VEL_NOISE_STD * hn.sn[4]; nz.v[2] = on * VEL_NOISE_STD * hn.sn[5];
+    nz.w[0] = on * GYRO_NOISE_STD * hn.sn[6]; nz.w[1] = on * GYRO_NOISE_STD * hn.sn[7]; nz.w[2] = on * GYRO_NOISE_STD * hn.sn[8];
+    return nz;
 }
 
 // One observation's noise under the custom model (qs_set_sensor_noise; add_noise_numba + add_noise_to_omega,

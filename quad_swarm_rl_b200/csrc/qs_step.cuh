@@ -299,10 +299,18 @@ __device__ __forceinline__ void emit_observation_tile(const StepParams& p, const
 // would otherwise put one ~20 k-instruction generator on the critical path of EVERY step.)
 struct EpisodeLane { V3 goal; ResetPose pose; int scn_next; float approach; float obst_r; };
 
-__device__ __forceinline__ RngKey episode_key(const StepParams& p, int env, int episode) {
+// key of the draws of env `env` in the step with the env's step counter `step`
+__device__ __forceinline__ RngKey step_key(const StepParams& p, int env, uint32_t step) {
     RngKey k;
     k.k0 = p.seed_lo; k.k1 = p.seed_hi;
     k.env = (uint32_t)(p.env_id_offset + env);
+    k.step = step;
+    return k;
+}
+
+// (the episode word is set last: as step_key's argument it is computed first, which changes the reset path's register allocation)
+__device__ __forceinline__ RngKey episode_key(const StepParams& p, int env, int episode) {
+    RngKey k = step_key(p, env, 0u);
     k.step = EPISODE_KEY_BIT | (uint32_t)episode;
     return k;
 }
@@ -510,6 +518,28 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, int parity) {
 // round trip per counter on the critical path of every warp with a discrete event.
 __device__ __forceinline__ void cnt_add(int32_t* c, int k, int v) { if (v != 0) atomicAdd(c + k, v); }
 
+// Polls a hand-over word with acquire loads while WAITING(value, want) holds, at most 2^24 times with a 40 ns back-off (~1 s:
+// a lost hand-over must not hang the GPU).  Returns whether it gave up.  A flag is waited for until it is set, a counter
+// until it reaches `want` (compared as a difference: the counters wrap around after 2^32 steps).
+__device__ __forceinline__ bool flag_unset(int v, int) { return v == 0; }
+__device__ __forceinline__ bool counter_below(int v, int want) { return v - want < 0; }
+template <bool (*WAITING)(int, int)>
+__device__ __forceinline__ bool poll_acquire(const int* word, int want) {
+    int v = 0, spins = 0;
+    do {
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(word) : "memory");
+        if (WAITING(v, want)) __nanosleep(40);
+    } while (WAITING(v, want) && ++spins < (1 << 24));
+    return WAITING(v, want);
+}
+// A hand-over that timed out: the env block is stepped from state that may be incomplete.  Counted (qs_handover_timeouts) and
+// latched in the handle's sticky error word: every later qs_step fails.
+__device__ __forceinline__ void report_handover_timeout(int* timeouts, int* err_flag) {
+    atomicAdd(timeouts, 1);
+    if (err_flag != nullptr) *reinterpret_cast<volatile int*>(err_flag) = 1;
+    __threadfence_system();
+}
+
 // ---- per-block hand-over between consecutive step grids (HO kernels) ----
 // Envs are independent, so block b of step t+1 only needs block b of step t.  Every step launch carries the programmatic
 // stream-serialization attribute; instead of griddepcontrol.wait (a grid-wide barrier: every step then costs the launch
@@ -520,16 +550,7 @@ __device__ __forceinline__ void cnt_add(int32_t* c, int k, int v) { if (v != 0) 
 // never triggers early, so it still sees, and is seen by, whole step grids.  (This flag protocol, run by thread 0, serves the
 // split and the multi-wave shapes; balanced single-wave grids use the counters of the courier warp below.)
 __device__ __forceinline__ void handover_acquire(int* ready, int* timeouts, int* err_flag) {
-    int v = 0, spins = 0;
-    do {
-        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(ready) : "memory");
-        if (v == 0) __nanosleep(40);
-    } while (v == 0 && ++spins < (1 << 24));          // ~1 s: a lost hand-over must not hang the GPU
-    if (v == 0) {                                     // the env block is stepped from state that may be incomplete:
-        atomicAdd(timeouts, 1);                       // counted (qs_handover_timeouts) and latched in the handle's sticky
-        if (err_flag != nullptr) *reinterpret_cast<volatile int*>(err_flag) = 1;      // error word: every later qs_step fails
-        __threadfence_system();
-    }
+    if (poll_acquire<flag_unset>(ready, 0)) report_handover_timeout(timeouts, err_flag);
     asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(ready), "r"(0) : "memory");
 }
 // st.release = fence + store (SASS: MEMBAR.ALL.GPU; STG.E.STRONG.GPU); an extra __threadfence() in front of it was a second,
@@ -554,17 +575,14 @@ __device__ __forceinline__ void handover_release(int* ready) {
 // At rest T = S = D and Tw = Dw = Rw; an unchained launch needs no special case.
 enum { HW_READY = 0, HW_T = 1, HW_S = 2, HW_D = 3, HW_TW = 4, HW_DW = 5, HW_RW = 6, HW_ROWS = 7 };     // rows of DevState::ready, [E + 1] each
 __device__ __forceinline__ int* hw_word(const DevState& st, int E, int row) { return st.ready + (long long)row * (E + 1) + blockIdx.x; }
+// poll_acquire<counter_below> written out: called through it, the NP = 32 hand-over step kernels compile to different code
 __device__ __forceinline__ void counter_wait(const int* c, int want, int* timeouts, int* err_flag) {
     int v = 0, spins = 0;
     do {
         asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(c) : "memory");
         if (v - want < 0) __nanosleep(40);
     } while (v - want < 0 && ++spins < (1 << 24));    // ~1 s: a lost hand-over must not hang the GPU
-    if (v - want < 0) {
-        atomicAdd(timeouts, 1);
-        if (err_flag != nullptr) *reinterpret_cast<volatile int*>(err_flag) = 1;
-        __threadfence_system();
-    }
+    if (v - want < 0) report_handover_timeout(timeouts, err_flag);
 }
 __device__ __forceinline__ void counter_set(int* c, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(c), "r"(v) : "memory"); }
 __device__ __forceinline__ void counter_inc(int* c) { asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(c), "r"(1) : "memory"); }
@@ -773,15 +791,7 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
             __syncwarp();
         }
     }
-    if (!valid) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { s.pos[k] = 1e9f + 1e6f * i; s.vel[k] = 0.f; s.om[k] = 0.f; s.goal[k] = 0.f; }
-#pragma unroll
-        for (int k = 0; k < 9; ++k) s.R[k] = (k % 4 == 0) ? 1.f : 0.f;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { s.rd[k] = 0.f; s.cd[k] = 0.f; s.ou[k] = 0.f; s.ring[k] = 0.f; }
-        s.flags = 0u; s.prev_col = 0u;
-    }
+    if (!valid) idle_agent(s, i);
     ctr.tick = ctr_raw.x; ctr.step_count = ctr_raw.y; ctr.svd_count = ctr_raw.z; ctr.episode_idx = ctr_raw.w;
 #ifdef QS_TIMELINE
     if (ctr.tick + __float_as_int(s.pos[0]) == 0x7fffffff) QS_TL(7);      // depends on the loaded state: stamp 2 follows the loads
@@ -795,19 +805,10 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
         const int envs_here = min(envs_per_block, p.E - env_first);
 #pragma unroll 1
         for (int t = 0; t < p.T; ++t) {
-            RngKey key;
-            key.k0 = p.seed_lo; key.k1 = p.seed_hi;
-            key.env = (uint32_t)(p.env_id_offset + env);
-            key.step = (uint32_t)ctr.step_count;
+            const RngKey key = step_key(p, env, ctr.step_count);
             const bool want = !p.last_obs_only || t == p.T - 1;
-            Noise9 nz;
-            {   // first sensor-noise draw (SITE_HOT, 2 Philox blocks), overlapped with the physics warp's integration
-                const HotNormals hn = hot_normals(key, i);
-                const float on = p.sense_noise ? 1.f : 0.f;
-                nz.p[0] = on * POS_NOISE_STD * hn.sn[0]; nz.p[1] = on * POS_NOISE_STD * hn.sn[1]; nz.p[2] = on * POS_NOISE_STD * hn.sn[2];
-                nz.v[0] = on * VEL_NOISE_STD * hn.sn[3]; nz.v[1] = on * VEL_NOISE_STD * hn.sn[4]; nz.v[2] = on * VEL_NOISE_STD * hn.sn[5];
-                nz.w[0] = on * GYRO_NOISE_STD * hn.sn[6]; nz.w[1] = on * GYRO_NOISE_STD * hn.sn[7]; nz.w[2] = on * GYRO_NOISE_STD * hn.sn[8];
-            }
+            // first sensor-noise draw (SITE_HOT, 2 Philox blocks), overlapped with the physics warp's integration
+            Noise9 nz = default_noise(hot_normals(key, i), p.sense_noise);
             Agent o;
             float nvel[3];
             bar_sync(1);                                              // post-integration state is in the hand-off arrays
@@ -853,10 +854,7 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
 
 #pragma unroll 1
     for (int t = 0; t < p.T; ++t) {
-        RngKey key;
-        key.k0 = p.seed_lo; key.k1 = p.seed_hi;
-        key.env = (uint32_t)(p.env_id_offset + env);
-        key.step = (uint32_t)ctr.step_count;
+        const RngKey key = step_key(p, env, ctr.step_count);
 
         // the draws every drone needs every step: OU thrust noise + first sensor-noise draw (SITE_HOT: 2 Philox blocks)
         Noise9 nz;
@@ -870,10 +868,7 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
         } else {
             const HotNormals hn = hot_normals(key, i);
             ou_z = make_float4(hn.ou[0], hn.ou[1], hn.ou[2], hn.ou[3]);
-            const float on = p.sense_noise ? 1.f : 0.f;
-            nz.p[0] = on * POS_NOISE_STD * hn.sn[0]; nz.p[1] = on * POS_NOISE_STD * hn.sn[1]; nz.p[2] = on * POS_NOISE_STD * hn.sn[2];
-            nz.v[0] = on * VEL_NOISE_STD * hn.sn[3]; nz.v[1] = on * VEL_NOISE_STD * hn.sn[4]; nz.v[2] = on * VEL_NOISE_STD * hn.sn[5];
-            nz.w[0] = on * GYRO_NOISE_STD * hn.sn[6]; nz.w[1] = on * GYRO_NOISE_STD * hn.sn[7]; nz.w[2] = on * GYRO_NOISE_STD * hn.sn[8];
+            nz = default_noise(hn, p.sense_noise);
             if (NZ) {
                 const SensedNoise sn = sensor_noise_model(p.nz, key, 0, i, gb, gyro_model);
                 nz = sn.n; gb = sn.bias;
@@ -1139,22 +1134,17 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
                 V3 pos = {s.pos[0], s.pos[1], s.pos[2]}, vel = {s.vel[0], s.vel[1], s.vel[2]};
                 const KickVO o = obstacle_response(key, i, pos, vel, ob.x, ob.y, 0.5f * (p.room_hi[2] - p.room_lo[2]) + p.room_lo[2],
                                                    obst_r);
-                s.vel[0] = o.vel.x; s.vel[1] = o.vel.y; s.vel[2] = o.vel.z;
-                s.om[0] += o.dom.x; s.om[1] += o.dom.y; s.om[2] += o.dom.z;
+                apply_kick(s, o);
             }
             if (wall_c) {
                 V3 vel = {s.vel[0], s.vel[1], s.vel[2]};
                 const int tx = s.pos[0] == p.room_lo[0] ? -1 : (s.pos[0] == p.room_hi[0] ? 1 : 0);
                 const int ty = s.pos[1] == p.room_lo[1] ? -1 : (s.pos[1] == p.room_hi[1] ? 1 : 0);
-                const KickVO o = wall_response(key, i, vel, tx, ty);
-                s.vel[0] = o.vel.x; s.vel[1] = o.vel.y; s.vel[2] = o.vel.z;
-                s.om[0] += o.dom.x; s.om[1] += o.dom.y; s.om[2] += o.dom.z;
+                apply_kick(s, wall_response(key, i, vel, tx, ty));
             }
             if (ceil_c) {
                 V3 vel = {s.vel[0], s.vel[1], s.vel[2]};
-                const KickVO o = ceiling_response(key, i, vel);
-                s.vel[0] = o.vel.x; s.vel[1] = o.vel.y; s.vel[2] = o.vel.z;
-                s.om[0] += o.dom.x; s.om[1] += o.dom.y; s.om[2] += o.dom.z;
+                apply_kick(s, ceiling_response(key, i, vel));
             }
             if (kicked) {
                 s.flags |= QS_FLAG_KICKED;
@@ -1382,24 +1372,13 @@ __global__ void __launch_bounds__(128) qs_reset_kernel(const __grid_constant__ S
 
     Agent s;
     if (valid) load_agent(st, a, s);
-    else {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { s.pos[k] = 1e9f + 1e6f * i; s.vel[k] = 0.f; s.om[k] = 0.f; s.goal[k] = 0.f; }
-#pragma unroll
-        for (int k = 0; k < 9; ++k) s.R[k] = (k % 4 == 0) ? 1.f : 0.f;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { s.rd[k] = 0.f; s.cd[k] = 0.f; s.ou[k] = 0.f; s.ring[k] = 0.f; }
-        s.flags = 0u; s.prev_col = 0u;
-    }
+    else idle_agent(s, i);
     EnvCtr ctr = {0, 0, 0, 0};
     if (env_ok) {
         const int4 c = st.env_ctr[env];
         ctr.tick = c.x; ctr.step_count = c.y; ctr.svd_count = c.z; ctr.episode_idx = c.w;
     }
-    RngKey key;
-    key.k0 = p.seed_lo; key.k1 = p.seed_hi;
-    key.env = (uint32_t)(p.env_id_offset + env);
-    key.step = (uint32_t)ctr.step_count;
+    const RngKey key = step_key(p, env, ctr.step_count);
     float nvel[3] = {0.f, 0.f, 0.f};
     // every lane of the warp takes part in the shuffles below; lanes of unmasked envs write nothing
     int scn_next = SCN_NEVER;

@@ -94,13 +94,7 @@ __device__ __forceinline__ void agg_add(float* agg, int k, float v) { if (v != 0
 // observation rows may still be on their way.  Called by whole warps right before they read or overwrite rows of q.obs.
 __device__ __forceinline__ void wait_rows(const WrapView& q) {
     if (q.rows == nullptr) return;
-    if ((threadIdx.x & 31) == 0) {
-        int v = 0, spins = 0;
-        do {
-            asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(q.rows) : "memory");
-            if (v - q.rows_want < 0) __nanosleep(40);
-        } while (v - q.rows_want < 0 && ++spins < (1 << 24));      // a lost count is caught (and reported) at the end of the kernel
-    }
+    if ((threadIdx.x & 31) == 0) poll_acquire<counter_below>(q.rows, q.rows_want);    // a lost count is caught (and reported) at the end of the kernel
     __syncwarp();
 }
 
@@ -413,9 +407,7 @@ __device__ __forceinline__ void wrap_body(const WrapView& q, int env, int i) {
             rq.x = 0;
             int n_valid = 0;
             for (int b = 0; b < w.buffer; ++b) n_valid += __ldcg(w.ev_state + (long long)env * w.buffer + b) >= 0 ? 1 : 0;
-            RngKey k2;
-            k2.k0 = p.seed_lo; k2.k1 = p.seed_hi; k2.env = (uint32_t)(p.env_id_offset + env); k2.step = (uint32_t)step_count;
-            const float4 u = rng_uniform4(k2, SITE_REPLAY_U, 0, 0, 0);
+            const float4 u = rng_uniform4(step_key(p, env, step_count), SITE_REPLAY_U, 0, 0, 0);
             if (n_valid > 0 && rq.y && u.x < w.replay_prob) {
                 int want = min((int)(u.y * (float)n_valid), n_valid - 1);
                 for (int b = 0; b < w.buffer; ++b) {
