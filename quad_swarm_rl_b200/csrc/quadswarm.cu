@@ -1,5 +1,6 @@
 // C ABI of the H100-native QuadSwarm env step (see include/quadswarm.h for the contract and the
 // reference interfaces each entry point replaces).  Build: nvcc -gencode arch=compute_90a,code=sm_90a.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -68,6 +69,9 @@ struct QsHandle {
     float *h_actions, *h_obs, *h_rewards, *h_terms;
     uint8_t *h_dones, *h_mask;
     cudaStream_t own_stream;
+    // every buffer above is one of these (dev_alloc / host_alloc): release_handle frees them whichever call failed
+    std::vector<void*> dev_bufs;     // device memory
+    std::vector<void*> host_bufs;    // page-locked host memory
 };
 
 static thread_local std::string g_err;
@@ -86,7 +90,48 @@ static int fail(int code, const std::string& msg) {
 
 extern "C" const char* qs_last_error(void) { return g_err.c_str(); }
 
-static inline int blocks_for(long long n) { return (int)((n + 255) / 256); }
+// Zero-filled device buffer owned by the handle.  *out is set only once the buffer is complete; a buffer whose fill
+// failed stays owned and is freed with the handle.
+template <typename T>
+static cudaError_t dev_alloc(QsHandle* h, T** out, size_t bytes) {
+    void* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) return e;
+    h->dev_bufs.push_back(p);
+    e = cudaMemset(p, 0, bytes);
+    if (e == cudaSuccess) *out = (T*)p;
+    return e;
+}
+
+// Page-locked host buffer (cudaHostAlloc flags) owned by the handle.
+template <typename T>
+static cudaError_t host_alloc(QsHandle* h, T** out, size_t bytes, unsigned flags) {
+    void* p = nullptr;
+    const cudaError_t e = cudaHostAlloc(&p, bytes, flags);
+    if (e != cudaSuccess) return e;
+    h->host_bufs.push_back(p);
+    *out = (T*)p;
+    return e;
+}
+
+// Frees a buffer of dev_alloc before the handle goes.
+static void dev_release(QsHandle* h, void* p) {
+    const auto it = std::find(h->dev_bufs.begin(), h->dev_bufs.end(), p);
+    if (it == h->dev_bufs.end()) return;
+    h->dev_bufs.erase(it);
+    cudaFree(p);
+}
+
+// Frees everything the handle owns, then the handle.  Leaves g_err alone: it runs after a failed qs_create, whose
+// message must survive.
+static void release_handle(QsHandle* h) {
+    cudaSetDevice(h->device);
+    for (void* p : h->dev_bufs) cudaFree(p);
+    for (void* p : h->host_bufs) cudaFreeHost(p);
+    if (h->own_stream) cudaStreamDestroy(h->own_stream);
+    if (h->ev_sync) cudaEventDestroy(h->ev_sync);
+    delete h;
+}
 
 static int next_pow2(int n) {
     int p = 1;
@@ -202,6 +247,23 @@ static void join_caller_stream(QsHandle* h) {
     cudaDeviceSynchronize();
 }
 
+// One thread per table entry (n of them) on the caller's stream: the launch of the table, state and statistics kernels.
+template <typename... P, typename... Args>
+static int launch_table(QsHandle* h, void* stream, long long n, void (*kernel)(P...), Args... args) {
+    QS_CUDA(cudaSetDevice(h->device));
+    kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(args...);
+    QS_CUDA(cudaGetLastError());
+    h->launches += 1;
+    note_async(h, (cudaStream_t)stream, false);
+    return QS_OK;
+}
+
+// Threads of the kernels that walk both the drones and the pillars: max(A, E * M).
+static long long agents_or_pillars(const QsHandle* h) {
+    const long long em = (long long)h->cfg.num_envs * h->M;
+    return h->A > em ? h->A : em;
+}
+
 // ------------------------------------------------------------------------------------------
 // small kernels: tables, goals, state import / export
 // ------------------------------------------------------------------------------------------
@@ -231,6 +293,28 @@ __global__ void k_set_goals(DevState st, int E, int N, const uint8_t* mask, cons
         st.slots[SL_GOAL * st.a_pad + t] = make_float4(goals[3 * t], goals[3 * t + 1], goals[3 * t + 2], 0.f);
 }
 
+// The QS_STATE_F32 row of a drone (engine.STATE_F32_FIELDS): the float fields of its Agent, then x, y, z of its distance
+// sums and of its stale velocity.  TO_ROW copies the drone into the row (k_get_state), else the row into the drone.
+template <bool TO_ROW, typename Row>
+__device__ __forceinline__ void map_state_row(Row* row, Agent& s, float4& sums, float4& stale) {
+    int k = 0;
+    const auto map = [&](float& v) {
+        if constexpr (TO_ROW) row[k++] = v;
+        else v = row[k++];
+    };
+    for (int c = 0; c < 3; ++c) map(s.pos[c]);
+    for (int c = 0; c < 3; ++c) map(s.vel[c]);
+    for (int c = 0; c < 9; ++c) map(s.R[c]);
+    for (int c = 0; c < 3; ++c) map(s.om[c]);
+    for (int c = 0; c < 4; ++c) map(s.rd[c]);
+    for (int c = 0; c < 4; ++c) map(s.cd[c]);
+    for (int c = 0; c < 4; ++c) map(s.ou[c]);
+    for (int c = 0; c < 3; ++c) map(s.goal[c]);
+    for (int c = 0; c < 4; ++c) map(s.ring[c]);
+    map(sums.x); map(sums.y); map(sums.z);
+    map(stale.x); map(stale.y); map(stale.z);
+}
+
 static_assert(QS_STATE_ENV_I32 >= 4 + QS_NUM_ENV_STATS + 17, "env state row too short");
 __global__ void k_get_state(DevState st, int E, int N, int M, float* af, uint32_t* au, int32_t* ei, float* obst) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -238,20 +322,8 @@ __global__ void k_get_state(DevState st, int E, int N, int M, float* af, uint32_
     if (t < A) {
         Agent s;
         load_agent(st, t, s);
-        float* o = af + t * QS_STATE_F32;
-        int k = 0;
-        for (int c = 0; c < 3; ++c) o[k++] = s.pos[c];
-        for (int c = 0; c < 3; ++c) o[k++] = s.vel[c];
-        for (int c = 0; c < 9; ++c) o[k++] = s.R[c];
-        for (int c = 0; c < 3; ++c) o[k++] = s.om[c];
-        for (int c = 0; c < 4; ++c) o[k++] = s.rd[c];
-        for (int c = 0; c < 4; ++c) o[k++] = s.cd[c];
-        for (int c = 0; c < 4; ++c) o[k++] = s.ou[c];
-        for (int c = 0; c < 3; ++c) o[k++] = s.goal[c];
-        for (int c = 0; c < 4; ++c) o[k++] = s.ring[c];
-        const float4 sums = st.slots[SL_DIST_SUMS * st.a_pad + t], sv = st.slots[SL_STALE_VEL * st.a_pad + t];
-        o[k++] = sums.x; o[k++] = sums.y; o[k++] = sums.z;
-        o[k++] = sv.x; o[k++] = sv.y; o[k++] = sv.z;
+        float4 sums = st.slots[SL_DIST_SUMS * st.a_pad + t], sv = st.slots[SL_STALE_VEL * st.a_pad + t];
+        map_state_row<true>(af + t * QS_STATE_F32, s, sums, sv);
         uint32_t* u = au + t * QS_STATE_U32;
         u[0] = s.flags; u[1] = s.prev_col; u[2] = 0u; u[3] = 0u;
     }
@@ -283,20 +355,10 @@ __global__ void k_set_state(DevState st, int E, int N, int M, const uint8_t* mas
     const long long A = (long long)E * N;
     if (t < A && (mask == nullptr || mask[t / N])) {
         Agent s;
-        const float* o = af + t * QS_STATE_F32;
-        int k = 0;
-        for (int c = 0; c < 3; ++c) s.pos[c] = o[k++];
-        for (int c = 0; c < 3; ++c) s.vel[c] = o[k++];
-        for (int c = 0; c < 9; ++c) s.R[c] = o[k++];
-        for (int c = 0; c < 3; ++c) s.om[c] = o[k++];
-        for (int c = 0; c < 4; ++c) s.rd[c] = o[k++];
-        for (int c = 0; c < 4; ++c) s.cd[c] = o[k++];
-        for (int c = 0; c < 4; ++c) s.ou[c] = o[k++];
-        for (int c = 0; c < 3; ++c) s.goal[c] = o[k++];
-        for (int c = 0; c < 4; ++c) s.ring[c] = o[k++];
-        st.slots[SL_DIST_SUMS * st.a_pad + t] = make_float4(o[k], o[k + 1], o[k + 2], 0.f);
-        k += 3;
-        st.slots[SL_STALE_VEL * st.a_pad + t] = make_float4(o[k], o[k + 1], o[k + 2], 0.f);
+        float4 sums = make_float4(0.f, 0.f, 0.f, 0.f), sv = sums;
+        map_state_row<false>(af + t * QS_STATE_F32, s, sums, sv);
+        st.slots[SL_DIST_SUMS * st.a_pad + t] = sums;
+        st.slots[SL_STALE_VEL * st.a_pad + t] = sv;
         const uint32_t* u = au + t * QS_STATE_U32;
         s.flags = u[0]; s.prev_col = u[1];
         store_agent(st, t, s, true);
@@ -507,7 +569,7 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     h->step_wrap_chain = p.wrap_chain;
     h->wrap_block = sh.work_threads;
 #ifdef QS_TIMELINE
-    if (!h->tl) { QS_CUDA(cudaMalloc((void**)&h->tl, sizeof(unsigned long long) * 64 * 4096 * 16)); QS_CUDA(cudaMemset(h->tl, 0, sizeof(unsigned long long) * 64 * 4096 * 16)); }
+    if (!h->tl) QS_CUDA(dev_alloc(h, &h->tl, sizeof(unsigned long long) * 64 * 4096 * 16));
     p.tl = h->tl; p.tl_slot = h->tl_next; h->tl_next = (h->tl_next + 1) % 64;
 #endif
     // Programmatic dependent launch between consecutive step grids: a grid-wide-wait kernel lets the next grid launch just
@@ -569,6 +631,67 @@ static int launch_reset(QsHandle* h, const StepParams& p, cudaStream_t s) {
     return QS_OK;
 }
 
+// The buffers of a new handle (qs_create).  On an error, what was allocated stays owned by the handle.
+static int alloc_buffers(QsHandle* h) {
+    DevState& st = h->st;
+    st.a_pad = h->a_pad;
+    const long long E = h->cfg.num_envs, A = h->A, M = h->M > 0 ? h->M : 1;
+    QS_CUDA(dev_alloc(h, &st.slots, sizeof(float4) * NUM_SLOTS * h->a_pad));
+    QS_CUDA(dev_alloc(h, &st.env_ctr, sizeof(int4) * E));
+    QS_CUDA(dev_alloc(h, &st.env_cnt, sizeof(int32_t) * E * QS_NUM_ENV_STATS));
+    QS_CUDA(dev_alloc(h, &st.obst, sizeof(float2) * E * M));
+    QS_CUDA(dev_alloc(h, &st.next_goal, sizeof(float4) * A));
+    QS_CUDA(dev_alloc(h, &st.next_spawn, sizeof(float4) * A));
+    QS_CUDA(dev_alloc(h, &st.next_obst, sizeof(float2) * E * M));
+    QS_CUDA(dev_alloc(h, &st.stats_env, sizeof(int32_t) * E * QS_NUM_ENV_STATS));
+    QS_CUDA(dev_alloc(h, &st.stats_agent, sizeof(float4) * A));
+    QS_CUDA(dev_alloc(h, &st.scn_i, sizeof(int4) * E));
+    QS_CUDA(dev_alloc(h, &st.scn_f, sizeof(float4) * 3 * E));
+    QS_CUDA(dev_alloc(h, &st.next_scn_i, sizeof(int4) * E));
+    QS_CUDA(dev_alloc(h, &st.next_scn_f, sizeof(float4) * 3 * E));
+    QS_CUDA(dev_alloc(h, &st.epi, sizeof(int2) * E));
+    {   // per-block hand-over words (at most one block per env), all "ready"
+        // hand-over words per block, [HW_ROWS][E + 1] (rows HW_*, qs_step.cuh): the `ready` flag of the thread-0 hand-over (1) and
+        // the courier warps' counters T, S, D, Tw, Dw, Rw (0); [0][E] is the time-out counter
+        QS_CUDA(dev_alloc(h, &st.ready, sizeof(int) * HW_ROWS * (E + 1)));
+        std::vector<int> init((size_t)HW_ROWS * (E + 1), 0);
+        for (long long k = 0; k < E; ++k) init[(size_t)k] = 1;
+        QS_CUDA(cudaMemcpy(st.ready, init.data(), sizeof(int) * HW_ROWS * (E + 1), cudaMemcpyHostToDevice));
+    }
+    // rotation = identity so that a never-reset env still holds a valid state: (omega.z, R00, R01, R02),
+    // (R10, R11, R12, R20), (R21, R22, flags, prev) all read (0, 1, 0, 0)
+    {
+        const std::vector<float4> id((size_t)h->a_pad, make_float4(0.f, 1.f, 0.f, 0.f));
+        for (const int slot : {SL_OM_R0, SL_R1_R20, SL_R2_FLAGS})
+            QS_CUDA(cudaMemcpy(st.slots + slot * h->a_pad, id.data(), sizeof(float4) * h->a_pad, cudaMemcpyHostToDevice));
+    }
+    // default episode table: every goal at (0, 0, 2), spawn at the goal (scenarios/base.py:137-139, static_same_goal)
+    {
+        const std::vector<float4> g((size_t)A, make_float4(0.f, 0.f, 2.f, 0.f));
+        QS_CUDA(cudaMemcpy(st.next_goal, g.data(), sizeof(float4) * A, cudaMemcpyHostToDevice));
+        QS_CUDA(cudaMemcpy(st.slots + SL_GOAL * h->a_pad, g.data(), sizeof(float4) * A, cudaMemcpyHostToDevice));
+    }
+    // staging buffers for the host entry points
+    QS_CUDA(dev_alloc(h, &h->d_actions, sizeof(float) * 4 * A));
+    QS_CUDA(dev_alloc(h, &h->d_obs, sizeof(float) * h->D * A));
+    QS_CUDA(dev_alloc(h, &h->d_rewards, sizeof(float) * A));
+    QS_CUDA(dev_alloc(h, &h->d_terms, sizeof(float) * QS_NUM_TERMS * A));
+    QS_CUDA(dev_alloc(h, &h->d_dones, A));
+    QS_CUDA(dev_alloc(h, &h->d_mask, E));
+    QS_CUDA(host_alloc(h, &h->h_actions, sizeof(float) * 4 * A, cudaHostAllocDefault));
+    QS_CUDA(host_alloc(h, &h->h_obs, sizeof(float) * h->D * A, cudaHostAllocDefault));
+    QS_CUDA(host_alloc(h, &h->h_rewards, sizeof(float) * A, cudaHostAllocDefault));
+    QS_CUDA(host_alloc(h, &h->h_terms, sizeof(float) * QS_NUM_TERMS * A, cudaHostAllocDefault));
+    QS_CUDA(host_alloc(h, &h->h_dones, A, cudaHostAllocDefault));
+    QS_CUDA(host_alloc(h, &h->h_mask, E, cudaHostAllocDefault));
+    QS_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
+    QS_CUDA(cudaEventCreateWithFlags(&h->ev_sync, cudaEventDisableTiming));
+    QS_CUDA(host_alloc(h, &h->err_host, sizeof(int), cudaHostAllocMapped));
+    *h->err_host = 0;
+    QS_CUDA(cudaHostGetDevicePointer((void**)&st.err_flag, h->err_host, 0));
+    return QS_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // API
 // ------------------------------------------------------------------------------------------
@@ -605,7 +728,6 @@ extern "C" int qs_create(const QsConfig* cfg, int device, QsHandle** out) {
     QS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     QsHandle* h = new (std::nothrow) QsHandle();
     if (!h) return fail(QS_ERR_INVALID_ARG, "out of host memory");
-    memset(h, 0, sizeof(*h));
     h->cfg = *cfg;
     h->device = device;
     h->sms = sms;
@@ -637,101 +759,17 @@ extern "C" int qs_create(const QsConfig* cfg, int device, QsHandle** out) {
     // QuadrotorEnvMulti defaults, quadrotor_multi.py:91-94
     const float def[QS_NUM_REW_COEFF] = {1.f, 0.05f, 1.f, 1.f, 0.1f, 5.f, 4.f, 5.f};
     memcpy(h->rew, def, sizeof(def));
-    DevState& st = h->st;
-    st.a_pad = h->a_pad;
-    const long long E = cfg->num_envs, A = h->A, M = h->M > 0 ? h->M : 1;
-#define QS_ALLOC0(ptr, bytes)                                     \
-    do {                                                          \
-        QS_CUDA(cudaMalloc((void**)&(ptr), (size_t)(bytes)));     \
-        QS_CUDA(cudaMemset((ptr), 0, (size_t)(bytes)));           \
-    } while (0)
-    QS_ALLOC0(st.slots, sizeof(float4) * NUM_SLOTS * h->a_pad);
-    QS_ALLOC0(st.env_ctr, sizeof(int4) * E);
-    QS_ALLOC0(st.env_cnt, sizeof(int32_t) * E * QS_NUM_ENV_STATS);
-    QS_ALLOC0(st.obst, sizeof(float2) * E * M);
-    QS_ALLOC0(st.next_goal, sizeof(float4) * A);
-    QS_ALLOC0(st.next_spawn, sizeof(float4) * A);
-    QS_ALLOC0(st.next_obst, sizeof(float2) * E * M);
-    QS_ALLOC0(st.stats_env, sizeof(int32_t) * E * QS_NUM_ENV_STATS);
-    QS_ALLOC0(st.stats_agent, sizeof(float4) * A);
-    QS_ALLOC0(st.scn_i, sizeof(int4) * E);
-    QS_ALLOC0(st.scn_f, sizeof(float4) * 3 * E);
-    QS_ALLOC0(st.next_scn_i, sizeof(int4) * E);
-    QS_ALLOC0(st.next_scn_f, sizeof(float4) * 3 * E);
-    QS_ALLOC0(st.epi, sizeof(int2) * E);
-    {   // per-block hand-over words (at most one block per env), all "ready"
-        // hand-over words per block, [HW_ROWS][E + 1] (rows HW_*, qs_step.cuh): the `ready` flag of the thread-0 hand-over (1) and
-        // the courier warps' counters T, S, D, Tw, Dw, Rw (0); [0][E] is the time-out counter
-        QS_CUDA(cudaMalloc((void**)&st.ready, sizeof(int) * HW_ROWS * (E + 1)));
-        std::vector<int> init((size_t)HW_ROWS * (E + 1), 0);
-        for (long long k = 0; k < E; ++k) init[(size_t)k] = 1;
-        QS_CUDA(cudaMemcpy(st.ready, init.data(), sizeof(int) * HW_ROWS * (E + 1), cudaMemcpyHostToDevice));
+    const int rc = alloc_buffers(h);
+    if (rc != QS_OK) {
+        release_handle(h);
+        return rc;
     }
-    // rotation = identity so that a never-reset env still holds a valid state
-    {
-        std::string tmp;
-        float4* init = (float4*)malloc(sizeof(float4) * h->a_pad);
-        for (long long a = 0; a < h->a_pad; ++a) init[a] = make_float4(0.f, 1.f, 0.f, 0.f);   // omega.z, R00, R01, R02
-        QS_CUDA(cudaMemcpy(st.slots + SL_OM_R0 * h->a_pad, init, sizeof(float4) * h->a_pad, cudaMemcpyHostToDevice));
-        for (long long a = 0; a < h->a_pad; ++a) init[a] = make_float4(0.f, 1.f, 0.f, 0.f);   // R10, R11, R12, R20
-        QS_CUDA(cudaMemcpy(st.slots + SL_R1_R20 * h->a_pad, init, sizeof(float4) * h->a_pad, cudaMemcpyHostToDevice));
-        for (long long a = 0; a < h->a_pad; ++a) init[a] = make_float4(0.f, 1.f, 0.f, 0.f);   // R21, R22, flags, prev
-        QS_CUDA(cudaMemcpy(st.slots + SL_R2_FLAGS * h->a_pad, init, sizeof(float4) * h->a_pad, cudaMemcpyHostToDevice));
-        free(init);
-    }
-    // default episode table: every goal at (0, 0, 2), spawn at the goal (scenarios/base.py:137-139, static_same_goal)
-    {
-        float4* g = (float4*)malloc(sizeof(float4) * A);
-        for (long long a = 0; a < A; ++a) g[a] = make_float4(0.f, 0.f, 2.f, 0.f);
-        QS_CUDA(cudaMemcpy(st.next_goal, g, sizeof(float4) * A, cudaMemcpyHostToDevice));
-        QS_CUDA(cudaMemcpy(st.slots + SL_GOAL * h->a_pad, g, sizeof(float4) * A, cudaMemcpyHostToDevice));
-        free(g);
-    }
-    // staging buffers for the host entry points
-    QS_CUDA(cudaMalloc((void**)&h->d_actions, sizeof(float) * 4 * A));
-    QS_CUDA(cudaMalloc((void**)&h->d_obs, sizeof(float) * h->D * A));
-    QS_CUDA(cudaMalloc((void**)&h->d_rewards, sizeof(float) * A));
-    QS_CUDA(cudaMalloc((void**)&h->d_terms, sizeof(float) * QS_NUM_TERMS * A));
-    QS_CUDA(cudaMalloc((void**)&h->d_dones, A));
-    QS_CUDA(cudaMalloc((void**)&h->d_mask, E));
-    QS_CUDA(cudaMallocHost((void**)&h->h_actions, sizeof(float) * 4 * A));
-    QS_CUDA(cudaMallocHost((void**)&h->h_obs, sizeof(float) * h->D * A));
-    QS_CUDA(cudaMallocHost((void**)&h->h_rewards, sizeof(float) * A));
-    QS_CUDA(cudaMallocHost((void**)&h->h_terms, sizeof(float) * QS_NUM_TERMS * A));
-    QS_CUDA(cudaMallocHost((void**)&h->h_dones, A));
-    QS_CUDA(cudaMallocHost((void**)&h->h_mask, E));
-    QS_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    QS_CUDA(cudaEventCreateWithFlags(&h->ev_sync, cudaEventDisableTiming));
-    QS_CUDA(cudaHostAlloc((void**)&h->err_host, sizeof(int), cudaHostAllocMapped));
-    *h->err_host = 0;
-    QS_CUDA(cudaHostGetDevicePointer((void**)&st.err_flag, h->err_host, 0));
     *out = h;
     return QS_OK;
 }
 
 extern "C" int qs_destroy(QsHandle* h) {
-    if (!h) return QS_OK;
-    cudaSetDevice(h->device);
-    DevState& st = h->st;
-    cudaFree(st.slots); cudaFree(st.env_ctr); cudaFree(st.env_cnt); cudaFree(st.obst); cudaFree(st.next_goal);
-    cudaFree(st.next_spawn); cudaFree(st.next_obst); cudaFree(st.stats_env); cudaFree(st.stats_agent);
-    cudaFree(st.dyn); cudaFree(st.next_dyn); cudaFree(st.dyn_pending);
-    cudaFree(st.scn_i); cudaFree(st.scn_f); cudaFree(st.ready); cudaFree(st.next_scn_i); cudaFree(st.next_scn_f); cudaFree(st.epi);
-    cudaFree(h->gyro_bias);
-    cudaFree(h->d_actions); cudaFree(h->d_obs); cudaFree(h->d_rewards); cudaFree(h->d_terms); cudaFree(h->d_dones);
-    cudaFree(h->d_mask);
-    cudaFreeHost(h->h_actions); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rewards); cudaFreeHost(h->h_terms);
-    cudaFreeHost(h->h_dones); cudaFreeHost(h->h_mask);
-    if (h->wrap_on) {
-        WrapState& w = h->wrap;
-        cudaFree(w.acc); cudaFree(w.ep_steps); cudaFree(w.true_reward); cudaFree(w.agg); cudaFree(w.snap_slots); cudaFree(w.snap_obs);
-        cudaFree(w.snap_env); cudaFree(w.snap_obst); cudaFree(w.rp); cudaFree(w.rq); cudaFree(w.crash_now); cudaFree(w.crash_hist);
-        cudaFree(w.ev_state); cudaFreeHost(h->wrap_agg_host);
-    }
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    if (h->ev_sync) cudaEventDestroy(h->ev_sync);
-    if (h->err_host) cudaFreeHost(h->err_host);
-    delete h;
+    if (h) release_handle(h);
     return QS_OK;
 }
 
@@ -773,26 +811,26 @@ extern "C" int qs_wrap_enable(QsHandle* h, const QsWrapConfig* cfg) {
     WrapState& w = h->wrap;
     memset(&w, 0, sizeof(w));
     const long long A = h->A, E = h->cfg.num_envs, N = h->cfg.num_agents, M = h->M > 0 ? h->M : 1;
-    QS_ALLOC0(w.acc, sizeof(float4) * 6 * A);
-    QS_ALLOC0(w.ep_steps, sizeof(int) * E);
-    QS_ALLOC0(w.true_reward, sizeof(float) * A);
-    QS_ALLOC0(w.agg, sizeof(float) * QS_WRAP_AGG);
-    QS_CUDA(cudaMallocHost((void**)&h->wrap_agg_host, sizeof(float) * QS_WRAP_AGG));
+    QS_CUDA(dev_alloc(h, &w.acc, sizeof(float4) * 6 * A));
+    QS_CUDA(dev_alloc(h, &w.ep_steps, sizeof(int) * E));
+    QS_CUDA(dev_alloc(h, &w.true_reward, sizeof(float) * A));
+    QS_CUDA(dev_alloc(h, &w.agg, sizeof(float) * QS_WRAP_AGG));
+    QS_CUDA(host_alloc(h, &h->wrap_agg_host, sizeof(float) * QS_WRAP_AGG, cudaHostAllocDefault));
     w.replay_on = cfg->use_replay ? 1 : 0;
     w.replay_prob = cfg->replay_prob;
     w.always_active = cfg->replay_always_active ? 1 : 0;
     if (w.replay_on) {
         w.buffer = cfg->replay_buffer_size;
         w.slots = RP_KEEP + w.buffer;
-        QS_ALLOC0(w.snap_slots, sizeof(float4) * E * w.slots * NUM_SLOTS * N);
-        QS_ALLOC0(w.snap_obs, sizeof(float) * E * w.slots * N * h->D);
-        QS_ALLOC0(w.snap_env, sizeof(int32_t) * E * w.slots * SNAP_ENV_I32);
-        QS_ALLOC0(w.snap_obst, sizeof(float2) * E * w.slots * M);
-        QS_ALLOC0(w.rp, sizeof(int4) * E);
-        QS_ALLOC0(w.rq, sizeof(int4) * E);
-        QS_ALLOC0(w.crash_now, sizeof(float) * E);
-        QS_ALLOC0(w.crash_hist, sizeof(float) * E * 100);
-        QS_CUDA(cudaMalloc((void**)&w.ev_state, sizeof(int32_t) * E * w.buffer));
+        QS_CUDA(dev_alloc(h, &w.snap_slots, sizeof(float4) * E * w.slots * NUM_SLOTS * N));
+        QS_CUDA(dev_alloc(h, &w.snap_obs, sizeof(float) * E * w.slots * N * h->D));
+        QS_CUDA(dev_alloc(h, &w.snap_env, sizeof(int32_t) * E * w.slots * SNAP_ENV_I32));
+        QS_CUDA(dev_alloc(h, &w.snap_obst, sizeof(float2) * E * w.slots * M));
+        QS_CUDA(dev_alloc(h, &w.rp, sizeof(int4) * E));
+        QS_CUDA(dev_alloc(h, &w.rq, sizeof(int4) * E));
+        QS_CUDA(dev_alloc(h, &w.crash_now, sizeof(float) * E));
+        QS_CUDA(dev_alloc(h, &w.crash_hist, sizeof(float) * E * 100));
+        QS_CUDA(dev_alloc(h, &w.ev_state, sizeof(int32_t) * E * w.buffer));
         QS_CUDA(cudaMemset(w.ev_state, 0xff, sizeof(int32_t) * E * w.buffer));          // -1: empty
         std::vector<int4> rp((size_t)E, make_int4(0, 0, 0, -(1 << 30)));
         QS_CUDA(cudaMemcpy(w.rp, rp.data(), sizeof(int4) * E, cudaMemcpyHostToDevice));
@@ -801,7 +839,7 @@ extern "C" int qs_wrap_enable(QsHandle* h, const QsWrapConfig* cfg) {
             QS_CUDA(cudaMemcpy(w.rq, rq.data(), sizeof(int4) * E, cudaMemcpyHostToDevice));
         }
     }
-    h->wrap_on = true;
+    h->wrap_on = true;      // last: after a failure the wrappers stay off (the buffers are the handle's all the same)
     return QS_OK;
 }
 
@@ -910,13 +948,12 @@ extern "C" int qs_set_obstacle_randomization(QsHandle* h, const float* densities
 extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const float* rows_dev, int at_next_reset, void* stream) {
     if (!h || !rows_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
     if (((uintptr_t)rows_dev & 15u) != 0) return fail(QS_ERR_INVALID_ARG, "rows must be 16-byte aligned");
-    QS_CUDA(cudaSetDevice(h->device));
     DevState& st = h->st;
     const long long A = h->A, E = h->cfg.num_envs;
     if (st.dyn == nullptr) {
         // first use: both tables start as Crazyflie rows (the constants compiled into the other kernels), so that envs
-        // outside a mask keep flying the default model
-        std::vector<float> row(QS_DYN_ROW, 0.f);
+        // outside a mask keep flying the default model.  They are published once all three are complete.
+        QS_CUDA(cudaSetDevice(h->device));
         const float cf[QS_DYN_ROW] = {MASS, INV_MASS, IXX, IYY, IZZ, INV_IXX, INV_IYY, INV_IZZ, THRUST_MAX, THRUST_MAX, THRUST_MAX, THRUST_MAX,
                                       TORQUE_MAX, TORQUE_MAX, TORQUE_MAX, TORQUE_MAX, PROP_ARM_XY, -PROP_ARM_XY, -PROP_ARM_XY, -PROP_ARM_XY,
                                       -PROP_ARM_XY, PROP_ARM_XY, PROP_ARM_XY, PROP_ARM_XY, 0.f, 0.f, 0.f, 0.f, MOTOR_TAU_UP, MOTOR_TAU_DOWN,
@@ -925,21 +962,16 @@ extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const f
         for (long long a = 0; a < A; ++a) memcpy(&all[(size_t)a * QS_DYN_ROW], cf, sizeof(cf));
         float4 *d0 = nullptr, *d1 = nullptr;
         int* pend = nullptr;
-        QS_CUDA(cudaMalloc((void**)&d0, sizeof(float) * QS_DYN_ROW * A));
-        QS_CUDA(cudaMalloc((void**)&d1, sizeof(float) * QS_DYN_ROW * A));
-        QS_CUDA(cudaMalloc((void**)&pend, sizeof(int) * E));
+        QS_CUDA(dev_alloc(h, &d0, sizeof(float) * QS_DYN_ROW * A));
+        QS_CUDA(dev_alloc(h, &d1, sizeof(float) * QS_DYN_ROW * A));
+        QS_CUDA(dev_alloc(h, &pend, sizeof(int) * E));
         QS_CUDA(cudaMemcpy(d0, all.data(), sizeof(float) * QS_DYN_ROW * A, cudaMemcpyHostToDevice));
         QS_CUDA(cudaMemcpy(d1, all.data(), sizeof(float) * QS_DYN_ROW * A, cudaMemcpyHostToDevice));
-        QS_CUDA(cudaMemset(pend, 0, sizeof(int) * E));
         st.dyn = d0; st.next_dyn = d1; st.dyn_pending = pend;
     }
     const long long n = A * (QS_DYN_ROW / 4);
-    k_set_dynamics<<<blocks_for(n > E ? n : E), 256, 0, (cudaStream_t)stream>>>(st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev,
-                                                                               (const float4*)rows_dev, at_next_reset ? 1 : 0);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, n > E ? n : E, k_set_dynamics, st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev,
+                        (const float4*)rows_dev, at_next_reset ? 1 : 0);
 }
 
 extern "C" int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega_max) {
@@ -988,10 +1020,10 @@ extern "C" int qs_set_sensor_noise(QsHandle* h, const QsSensorNoise* sn) {
         m.random_walk = (float)sn->gyro_random_walk;
         if (h->gyro_bias == nullptr) {
             QS_CUDA(cudaSetDevice(h->device));
-            QS_ALLOC0(h->gyro_bias, sizeof(float4) * h->A);
+            QS_CUDA(dev_alloc(h, &h->gyro_bias, sizeof(float4) * h->A));
         }
     } else if (h->gyro_bias != nullptr) {
-        cudaFree(h->gyro_bias);
+        dev_release(h, h->gyro_bias);
         h->gyro_bias = nullptr;
     }
     h->nz = m;
@@ -1012,23 +1044,13 @@ __global__ void k_gyro_bias(float4* bias, long long A, int N, const uint8_t* mas
 
 extern "C" int qs_get_gyro_bias(QsHandle* h, float* bias_dev, void* stream) {
     if (!h || !bias_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
-    QS_CUDA(cudaSetDevice(h->device));
-    k_gyro_bias<<<blocks_for(h->A), 256, 0, (cudaStream_t)stream>>>(h->gyro_bias, h->A, h->cfg.num_agents, nullptr, bias_dev, nullptr);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, h->A, k_gyro_bias, h->gyro_bias, h->A, h->cfg.num_agents, nullptr, bias_dev, nullptr);
 }
 
 extern "C" int qs_set_gyro_bias(QsHandle* h, const uint8_t* env_mask_dev, const float* bias_dev, void* stream) {
     if (!h || !bias_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
     if (h->gyro_bias == nullptr) return fail(QS_ERR_INVALID_ARG, "the gyro bias model is off (qs_set_sensor_noise, gyro_norm_std)");
-    QS_CUDA(cudaSetDevice(h->device));
-    k_gyro_bias<<<blocks_for(h->A), 256, 0, (cudaStream_t)stream>>>(h->gyro_bias, h->A, h->cfg.num_agents, env_mask_dev, nullptr, bias_dev);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, h->A, k_gyro_bias, h->gyro_bias, h->A, h->cfg.num_agents, env_mask_dev, nullptr, bias_dev);
 }
 
 extern "C" int qs_set_reward_coeffs(QsHandle* h, const float* coeffs_host) {
@@ -1045,25 +1067,13 @@ extern "C" int qs_set_next_episode(QsHandle* h, const uint8_t* env_mask_dev, con
                                    const float* obst_xy_dev, void* stream) {
     if (!h || !goals_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
     if (obst_xy_dev && !h->cfg.use_obstacles) return fail(QS_ERR_INVALID_ARG, "obstacle table given but use_obstacles = 0");
-    QS_CUDA(cudaSetDevice(h->device));
-    const long long n = h->A > (long long)h->cfg.num_envs * h->M ? h->A : (long long)h->cfg.num_envs * h->M;
-    k_set_next_episode<<<blocks_for(n), 256, 0, (cudaStream_t)stream>>>(h->st, h->cfg.num_envs, h->cfg.num_agents, h->M,
-                                                                         env_mask_dev, goals_dev, spawn_dev, obst_xy_dev);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, agents_or_pillars(h), k_set_next_episode, h->st, h->cfg.num_envs, h->cfg.num_agents, h->M,
+                        env_mask_dev, goals_dev, spawn_dev, obst_xy_dev);
 }
 
 extern "C" int qs_set_goals(QsHandle* h, const uint8_t* env_mask_dev, const float* goals_dev, void* stream) {
     if (!h || !goals_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
-    QS_CUDA(cudaSetDevice(h->device));
-    k_set_goals<<<blocks_for(h->A), 256, 0, (cudaStream_t)stream>>>(h->st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev,
-                                                                     goals_dev);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, h->A, k_set_goals, h->st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev, goals_dev);
 }
 
 extern "C" int qs_reset(QsHandle* h, const uint8_t* env_mask_dev, float* obs_dev, void* stream) {
@@ -1222,38 +1232,20 @@ extern "C" int qs_reset_host(QsHandle* h, const uint8_t* env_mask_host, float* o
 extern "C" int qs_get_state(QsHandle* h, float* agent_f32_dev, uint32_t* agent_u32_dev, int32_t* env_i32_dev,
                             float* obst_xy_dev, void* stream) {
     if (!h || !agent_f32_dev || !agent_u32_dev || !env_i32_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
-    QS_CUDA(cudaSetDevice(h->device));
-    const long long n = h->A > (long long)h->cfg.num_envs * h->M ? h->A : (long long)h->cfg.num_envs * h->M;
-    k_get_state<<<blocks_for(n), 256, 0, (cudaStream_t)stream>>>(h->st, h->cfg.num_envs, h->cfg.num_agents, h->M, agent_f32_dev,
-                                                                  agent_u32_dev, env_i32_dev, h->M > 0 ? obst_xy_dev : nullptr);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, agents_or_pillars(h), k_get_state, h->st, h->cfg.num_envs, h->cfg.num_agents, h->M, agent_f32_dev,
+                        agent_u32_dev, env_i32_dev, h->M > 0 ? obst_xy_dev : nullptr);
 }
 
 extern "C" int qs_set_state(QsHandle* h, const uint8_t* env_mask_dev, const float* agent_f32_dev, const uint32_t* agent_u32_dev,
                             const int32_t* env_i32_dev, const float* obst_xy_dev, void* stream) {
     if (!h || !agent_f32_dev || !agent_u32_dev || !env_i32_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
-    QS_CUDA(cudaSetDevice(h->device));
-    const long long n = h->A > (long long)h->cfg.num_envs * h->M ? h->A : (long long)h->cfg.num_envs * h->M;
-    k_set_state<<<blocks_for(n), 256, 0, (cudaStream_t)stream>>>(h->st, h->cfg.num_envs, h->cfg.num_agents, h->M, env_mask_dev,
-                                                                  agent_f32_dev, agent_u32_dev, env_i32_dev,
-                                                                  h->M > 0 ? obst_xy_dev : nullptr);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, agents_or_pillars(h), k_set_state, h->st, h->cfg.num_envs, h->cfg.num_agents, h->M, env_mask_dev,
+                        agent_f32_dev, agent_u32_dev, env_i32_dev, h->M > 0 ? obst_xy_dev : nullptr);
 }
 
 extern "C" int qs_read_episode_stats(QsHandle* h, int32_t* env_stats_dev, float* agent_stats_dev, void* stream) {
     if (!h) return fail(QS_ERR_INVALID_ARG, "null argument");
-    QS_CUDA(cudaSetDevice(h->device));
     const long long n1 = h->A, n2 = (long long)h->cfg.num_envs * QS_NUM_ENV_STATS;
-    k_read_stats<<<blocks_for(n1 > n2 ? n1 : n2), 256, 0, (cudaStream_t)stream>>>(h->st, h->cfg.num_envs, h->cfg.num_agents,
-                                                                                   env_stats_dev, agent_stats_dev);
-    QS_CUDA(cudaGetLastError());
-    h->launches += 1;
-    note_async(h, (cudaStream_t)stream, false);
-    return QS_OK;
+    return launch_table(h, stream, n1 > n2 ? n1 : n2, k_read_stats, h->st, h->cfg.num_envs, h->cfg.num_agents, env_stats_dev,
+                        agent_stats_dev);
 }
