@@ -310,6 +310,25 @@ int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega
  * Works in every step shape. */
 int qs_set_numpy_dynamics(QsHandle* h, int enable);
 
+/* Control mode — replaces QuadrotorEnvMulti(raw_control=..., raw_control_zero_middle=...) (quadrotor_single.py:259-273):
+ *   QS_CONTROL_RAW (default): RawControl(zero_action_middle=True), motor command 0.5 (clip(action, -1, 1) + 1)
+ *     (quadrotor_control.py:37-57);
+ *   QS_CONTROL_RAW_UNIT: RawControl(zero_action_middle=False), motor command clip(action, 0, 1) (scale 1, bias 0, :37-49);
+ *   QS_CONTROL_POSITION: NonlinearPositionController with tf_control = False (:253-330), the Mellinger controller.  It
+ *     ignores the action and flies each drone to its current goal from the state at the start of the control step: the
+ *     desired acceleration 4.5 clamp_norm(goal - pos, 4) - 3.5 vel + (0, 0, g), the attitude error against the thrust
+ *     direction with the body x-axis towards (1, 0, 0), torques -200 e_R - 50 omega, and motor commands
+ *     clip(Jinv (thrust, torques), 0, 1) with Jinv = inv(quadrotor_jacobian(dynamics)) (:157-171) of each drone's
+ *     constants (the Crazyflie set, or the rows of qs_set_dynamics).
+ * Rewards and the wrapper statistics keep seeing the caller's raw action in every mode (quadrotor_single.py:347-349).
+ * Steps with a mode other than QS_CONTROL_RAW run in the single-warp shape with the grid-wide wait, on either dynamics path.
+ * Call after qs_create and before the first qs_reset / qs_step; later calls and unknown modes fail with QS_ERR_INVALID_ARG
+ * (the reference fixes the controller in its constructor). */
+#define QS_CONTROL_RAW 0
+#define QS_CONTROL_RAW_UNIT 1
+#define QS_CONTROL_POSITION 2
+int qs_set_control(QsHandle* h, int mode);
+
 /* flag bits in agent_u32[.,0] */
 #define QS_FLAG_ON_FLOOR (1u << 0)
 #define QS_FLAG_CRASHED_FLOOR (1u << 1)

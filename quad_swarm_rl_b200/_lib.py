@@ -19,6 +19,7 @@ QS_STATE_U32 = 4
 QS_STATE_ENV_I32 = 36
 QS_MAX_AGENTS = 32
 QS_DYN_ROW = 40
+QS_CONTROL_RAW, QS_CONTROL_RAW_UNIT, QS_CONTROL_POSITION = 0, 1, 2
 SCENARIO_HOST_TABLES, SCENARIO_O_RANDOM = 0, 1
 # scenarios with a device-side generator (QS_SCENARIO_* of include/quadswarm.h), by their reference names
 DEVICE_SCENARIOS = {'o_random': 1, 'static_same_goal': 2, 'static_diff_goal': 3, 'dynamic_same_goal': 4,
@@ -102,6 +103,7 @@ EXPORTS = {
     'qs_set_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_init_random_state': (C.c_int, [C.c_void_p, C.c_int, C.c_float, C.c_float]),
     'qs_set_numpy_dynamics': (C.c_int, [C.c_void_p, C.c_int]),
+    'qs_set_control': (C.c_int, [C.c_void_p, C.c_int]),
     'qs_wrap_enable': (C.c_int, [C.c_void_p, C.POINTER(QsWrapConfig)]),
     'qs_wrap_step': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_wrap_apply': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -44,6 +44,11 @@ constexpr float FLOOR_MU = 0.6f;
 #if QS_NUMPY_DYNAMICS
 constexpr float FLOOR_THRESHOLD_NP = 0.05f;       // floor threshold and snap height of the numpy path, every model (:75)
 #endif
+// QS_CONTROL_MODES = 1 (set by qs_step_pc.cu only): the step maps actions to motor commands by StepParams.control
+// (QS_CONTROL_RAW_UNIT or QS_CONTROL_POSITION, position_control() below) instead of RawControl with zero_action_middle.
+#ifndef QS_CONTROL_MODES
+#define QS_CONTROL_MODES 0
+#endif
 constexpr float SIM_DT = 0.005f;                  // quadrotor_single.py:157
 constexpr float CONTROL_DT = 0.01f;               // quadrotor_multi.py:83
 constexpr int SIM_STEPS = 2;                      // quadrotor_single.py:102
@@ -151,6 +156,7 @@ struct StepParams {
                                         // (not in DevState: the scenario functions take that by value)
     int init_random;                    // qs_set_init_random_state: every spawn gets a random vel / omega / R (random_init_state)
     float init_vel_max, init_omega_max;
+    int control;                        // qs_set_control: QS_CONTROL_*; read only by the kernels of qs_step_pc.cu
 };
 
 struct Agent {
@@ -314,6 +320,92 @@ __device__ __forceinline__ void load_phys(const float4* rows, long long a, Phys&
     ph.c_drag = q8.x; ph.c_roll = q8.y; ph.vel_damp = q8.z; ph.omega_quadratic = q8.w;
     ph.arm = q9.x;
 }
+
+#if QS_CONTROL_MODES
+// inv(quadrotor_jacobian(dynamics)) (quadrotor_control.py:157-171, :257-258), in float64 like np.linalg.inv.  J maps the
+// normalised motor thrusts to (acceleration along the body z-axis, angular accelerations):
+//   J[0][k] = thrust_max_k / mass, J[1][k] = thrust_max_k py_k / Ixx, J[2][k] = -thrust_max_k px_k / Iyy,
+//   J[3][k] = torque_max_k prop_ccw_k / Izz, prop_ccw = (-1, 1, -1, 1) (quadrotor_dynamics.py:47).
+// DYN = false: the compile-time Crazyflie constants (the compiler folds the inverse); DYN = true: the drone's row, so a row
+// latched at a reset is inverted from the next step on.  The inverse is the adjugate over the determinant: J of an
+// X-frame has zero leading minors, which Gauss-Jordan elimination would have to pivot around.
+template <bool DYN>
+__device__ __forceinline__ void jacobian_inverse(const Phys& ph, double Ji[16]) {
+    constexpr float CF_PX[4] = {PROP_ARM_XY, -PROP_ARM_XY, -PROP_ARM_XY, PROP_ARM_XY};
+    constexpr float CF_PY[4] = {-PROP_ARM_XY, -PROP_ARM_XY, PROP_ARM_XY, PROP_ARM_XY};
+    double m[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const double tm = DYN ? ph.thrust_max[k] : THRUST_MAX, qm = DYN ? ph.torque_max[k] : TORQUE_MAX;
+        const double px = DYN ? ph.px[k] : CF_PX[k], py = DYN ? ph.py[k] : CF_PY[k];
+        m[0][k] = tm / (double)(DYN ? ph.mass : MASS);
+        m[1][k] = tm * py / (double)(DYN ? ph.ixx : IXX);
+        m[2][k] = -tm * px / (double)(DYN ? ph.iyy : IYY);
+        m[3][k] = ((k & 1) ? qm : -qm) / (double)(DYN ? ph.izz : IZZ);
+    }
+    // 2 x 2 minors of rows 0-1 (s) and rows 2-3 (c)
+    const double s0 = m[0][0] * m[1][1] - m[1][0] * m[0][1], s1 = m[0][0] * m[1][2] - m[1][0] * m[0][2];
+    const double s2 = m[0][0] * m[1][3] - m[1][0] * m[0][3], s3 = m[0][1] * m[1][2] - m[1][1] * m[0][2];
+    const double s4 = m[0][1] * m[1][3] - m[1][1] * m[0][3], s5 = m[0][2] * m[1][3] - m[1][2] * m[0][3];
+    const double c5 = m[2][2] * m[3][3] - m[3][2] * m[2][3], c4 = m[2][1] * m[3][3] - m[3][1] * m[2][3];
+    const double c3 = m[2][1] * m[3][2] - m[3][1] * m[2][2], c2 = m[2][0] * m[3][3] - m[3][0] * m[2][3];
+    const double c1 = m[2][0] * m[3][2] - m[3][0] * m[2][2], c0 = m[2][0] * m[3][1] - m[3][0] * m[2][1];
+    const double inv_det = 1.0 / (s0 * c5 - s1 * c4 + s2 * c3 + s3 * c2 - s4 * c1 + s5 * c0);
+    Ji[0] = (m[1][1] * c5 - m[1][2] * c4 + m[1][3] * c3) * inv_det;
+    Ji[1] = (-m[0][1] * c5 + m[0][2] * c4 - m[0][3] * c3) * inv_det;
+    Ji[2] = (m[3][1] * s5 - m[3][2] * s4 + m[3][3] * s3) * inv_det;
+    Ji[3] = (-m[2][1] * s5 + m[2][2] * s4 - m[2][3] * s3) * inv_det;
+    Ji[4] = (-m[1][0] * c5 + m[1][2] * c2 - m[1][3] * c1) * inv_det;
+    Ji[5] = (m[0][0] * c5 - m[0][2] * c2 + m[0][3] * c1) * inv_det;
+    Ji[6] = (-m[3][0] * s5 + m[3][2] * s2 - m[3][3] * s1) * inv_det;
+    Ji[7] = (m[2][0] * s5 - m[2][2] * s2 + m[2][3] * s1) * inv_det;
+    Ji[8] = (m[1][0] * c4 - m[1][1] * c2 + m[1][3] * c0) * inv_det;
+    Ji[9] = (-m[0][0] * c4 + m[0][1] * c2 - m[0][3] * c0) * inv_det;
+    Ji[10] = (m[3][0] * s4 - m[3][1] * s2 + m[3][3] * s0) * inv_det;
+    Ji[11] = (-m[2][0] * s4 + m[2][1] * s2 - m[2][3] * s0) * inv_det;
+    Ji[12] = (-m[1][0] * c3 + m[1][1] * c1 - m[1][2] * c0) * inv_det;
+    Ji[13] = (m[0][0] * c3 - m[0][1] * c1 + m[0][2] * c0) * inv_det;
+    Ji[14] = (-m[3][0] * s3 + m[3][1] * s1 - m[3][2] * s0) * inv_det;
+    Ji[15] = (m[2][0] * s3 - m[2][1] * s1 + m[2][2] * s0) * inv_det;
+}
+
+// normalize(), quad_utils.py:80-86: x / |x|, or x unchanged when |x| < 1e-5
+__device__ __forceinline__ void normalize3(float v[3]) {
+    const float n = norm3(v[0], v[1], v[2]);
+    if (n >= 1e-5f) { v[0] /= n; v[1] /= n; v[2] /= n; }
+}
+
+// NonlinearPositionController.step, quadrotor_control.py:282-330 (tf_control = False): the motor commands that fly the drone
+// towards its goal, from its state at the start of the control step.  The action is not read.
+template <bool DYN>
+__device__ __forceinline__ void position_control(const Agent& s, const Phys& ph, float cmd[4]) {
+    float acc[3] = {s.goal[0] - s.pos[0], s.goal[1] - s.pos[1], s.goal[2] - s.pos[2]};
+    const float gd = norm3(acc[0], acc[1], acc[2]);
+    const float sc = gd <= 4.f ? 1.f : 4.f / gd;                             // -e_p = clamp_norm(goal - pos, 4.0), :287
+#pragma unroll
+    for (int k = 0; k < 3; ++k) acc[k] = 4.5f * (sc * acc[k]) - 3.5f * s.vel[k];   // kp_p = 4.5, kd_p = 3.5, :266, :290
+    acc[2] += GRAV;
+    float zb[3] = {acc[0], acc[1], acc[2]};
+    normalize3(zb);
+    float yb[3] = {0.f, zb[2], -zb[1]};                                       // cross(zb, rot_des[:, 0] = (1, 0, 0))
+    normalize3(yb);
+    const float xb[3] = {yb[1] * zb[2] - yb[2] * zb[1], yb[2] * zb[0] - yb[0] * zb[2], yb[0] * zb[1] - yb[1] * zb[0]};
+    // e_R = 0.5 vee(R_des^T R - R^T R_des); with A = R_des^T R, A_ij = (column i of R_des) . (column j of R)
+    auto rcol = [&](const float d[3], int j) { return d[0] * s.R[j] + d[1] * s.R[3 + j] + d[2] * s.R[6 + j]; };
+    const float e0 = 0.5f * (rcol(zb, 1) - rcol(yb, 2));
+    const float e1 = 0.5f * (rcol(xb, 2) - rcol(zb, 0));
+    const float e2 = 0.2f * (0.5f * (rcol(yb, 0) - rcol(xb, 1)));              // e_R[2] *= 0.2, :315
+    const float des[4] = {acc[0] * s.R[2] + acc[1] * s.R[5] + acc[2] * s.R[8],   // thrust_mag = acc_des . R[:, 2], :320
+                          -200.f * e0 - 50.f * s.om[0], -200.f * e1 - 50.f * s.om[1], -200.f * e2 - 50.f * s.om[2]};
+    double Ji[16];
+    jacobian_inverse<DYN>(ph, Ji);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const double t = Ji[4 * r] * des[0] + Ji[4 * r + 1] * des[1] + Ji[4 * r + 2] * des[2] + Ji[4 * r + 3] * des[3];
+        cmd[r] = clampf((float)t, 0.f, 1.f);                                   // :325-327
+    }
+}
+#endif
 
 // One 5 ms physics sub-step of the njit path: step1_numba, quadrotor_dynamics.py:348-383
 // (calculate_torque_integrate_rotations_and_update_omega :497-566, room clip :360-367,

@@ -623,7 +623,8 @@ __device__ __forceinline__ void hand_load(const float* hand, int lane, Agent& s,
 // NZ = true: the custom sensor-noise model (qs_set_sensor_noise, p.nz) instead of the compile-time 'default' set; the gyro
 // bias (p.gyro_bias, when that model is on) rides in registers across the steps of a launch.  Same shape as DYN.
 // qs_step_npy.cu compiles this kernel once more, as qs_step_kernel_npy, with the floor model of the reference's numpy path
-// (QS_NUMPY_DYNAMICS, qs_set_numpy_dynamics).
+// (QS_NUMPY_DYNAMICS, qs_set_numpy_dynamics).  qs_step_pc.cu / qs_step_pc_npy.cu compile it as qs_step_kernel_pc /
+// qs_step_kernel_pc_npy with the control modes of qs_set_control (QS_CONTROL_MODES).
 template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false, bool NZ = false>
 __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>()) qs_step_kernel(const __grid_constant__ StepParams p) {
     static_assert(!NZ || (!SPLIT && !HO), "the custom sensor-noise model runs in the single-warp shape with the grid-wide wait");
@@ -885,8 +886,17 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
         }
         av0 = make_float4(0.f, 0.f, 0.f, 0.f);         // used by the first step only: not live across the rest of the loop
         float cmd[4];
+#if QS_CONTROL_MODES
+        if (p.control == QS_CONTROL_POSITION) {                     // warp-uniform (one mode per handle)
+            position_control<DYN>(s, ph, cmd);
+        } else {
+#pragma unroll
+            for (int m = 0; m < 4; ++m) cmd[m] = clampf(act[m], 0.f, 1.f);    // RawControl(zero_action_middle=False), :37-57
+        }
+#else
 #pragma unroll
         for (int m = 0; m < 4; ++m) cmd[m] = 0.5f * (clampf(act[m], -1.f, 1.f) + 1.f);    // RawControl.step, quadrotor_control.py:53-57
+#endif
         // OU thrust noise, once per control step (numba_utils.py:101-105, quadrotor_dynamics.py:209)
         const float ou_sigma = DYN ? ph.ou_sigma : OU_SIGMA;
         s.ou[0] += OU_THETA * (0.f - s.ou[0]) + ou_sigma * ou_z.x;

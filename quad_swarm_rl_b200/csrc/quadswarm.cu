@@ -61,6 +61,7 @@ struct QsHandle {
     int init_random;      // qs_set_init_random_state
     float init_vel_max, init_omega_max;
     int numpy_dyn;        // qs_set_numpy_dynamics
+    int control;          // qs_set_control: QS_CONTROL_*
     cudaStream_t last_stream;   // stream of the most recent asynchronous call of this handle
     bool async_pending;
     // staging for the *_host entry points (pinned host + device mirrors)
@@ -182,6 +183,7 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.nz = h->nz;
     p.gyro_bias = h->gyro_bias;
     p.init_random = h->init_random; p.init_vel_max = h->init_vel_max; p.init_omega_max = h->init_omega_max;
+    p.control = h->control;
 }
 
 // Observation write-out mode of a step launch (qs_step.cuh, emit_observation_tile): the bulk-copy engine needs a 16-byte
@@ -423,6 +425,14 @@ static int dispatch_np(int NP, F&& f) {
 namespace qs_npy {
 void* step_kernel_npy(int NP, bool split, bool scn, bool ho, bool dyn, bool nz);
 }
+// The step kernels of the control modes of qs_set_control (qs_step_pc.cu, qs_step_pc_npy.cu): single-warp shape with the
+// grid-wide wait only.
+namespace qs_pc {
+void* step_kernel_pc(int NP, bool scn, bool dyn, bool nz);
+}
+namespace qs_pc_npy {
+void* step_kernel_pc(int NP, bool scn, bool dyn, bool nz);
+}
 
 struct StepShape {
     KernelFn fn;
@@ -478,13 +488,14 @@ static int courier_workers(QsHandle* h, KernelFn fn, int wpc_even) {
 static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const int NP = h->NP, sms = h->sms;
     const bool dyn = h->st.dyn != nullptr, nz = h->nz_on;
+    const bool ctl = h->control != QS_CONTROL_RAW;          // qs_set_control: like dyn / nz, single-warp shape, grid-wide wait
     const long long phys_warps = ((long long)h->cfg.num_envs * NP + 31) / 32;
     int wpc = (int)((phys_warps + sms - 1) / sms);          // worker warps per CTA of a balanced grid
     const bool balance_fits = NP < 16 && wpc >= 2 && wpc * 32 <= QS_LB && (wpc * 32) % NP == 0;
     const bool courier_fits = balance_fits && (wpc + 1) * 32 <= QS_LB;
-    const bool courier_shape = h->chained && !dyn && !nz && courier_fits;
+    const bool courier_shape = h->chained && !dyn && !nz && !ctl && courier_fits;
     const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
-    s.split = want_split && p.obs_stage && NP > 1 && !dyn && !nz && !h->obst_random;
+    s.split = want_split && p.obs_stage && NP > 1 && !dyn && !nz && !ctl && !h->obst_random;
     const bool balanced = !s.split && balance_fits;
     const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
     const bool scn = p.use_obst ? ticked_obst
@@ -492,6 +503,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
                                    p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
     auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
         KernelFn fn = nullptr;
+        if (ctl) return (KernelFn)(h->numpy_dyn ? qs_pc_npy::step_kernel_pc(NP, scn, k_dyn, k_nz) : qs_pc::step_kernel_pc(NP, scn, k_dyn, k_nz));
         if (h->numpy_dyn) return (KernelFn)qs_npy::step_kernel_npy(NP, s.split, scn, ho, k_dyn, k_nz);      // qs_set_numpy_dynamics
         dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
         return fn;
@@ -537,7 +549,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     if (balanced && s.smem < pad) s.smem = pad;
     // The hand-over kernels pay off only between step grids that follow each other directly; an unchained handle uses the
     // grid-wide wait (formally safe after any predecessor) and never pre-fetches across the dependency wait.
-    s.ho = h->handover == 1 && h->chained && !dyn && !nz;
+    s.ho = h->handover == 1 && h->chained && !dyn && !nz && !ctl;
     s.fn = kernel(s.ho, dyn, nz);
     return QS_OK;
 }
@@ -989,6 +1001,15 @@ extern "C" int qs_set_numpy_dynamics(QsHandle* h, int enable) {
     if (!h) return fail(QS_ERR_INVALID_ARG, "null argument");
     if (h->started) return fail(QS_ERR_INVALID_ARG, "the dynamics path can only be set before the first reset or step");
     h->numpy_dyn = enable ? 1 : 0;
+    return QS_OK;
+}
+
+extern "C" int qs_set_control(QsHandle* h, int mode) {
+    if (!h) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->started) return fail(QS_ERR_INVALID_ARG, "the control mode can only be set before the first reset or step");
+    if (mode != QS_CONTROL_RAW && mode != QS_CONTROL_RAW_UNIT && mode != QS_CONTROL_POSITION)
+        return fail(QS_ERR_INVALID_ARG, "unknown control mode (QS_CONTROL_RAW, QS_CONTROL_RAW_UNIT or QS_CONTROL_POSITION)");
+    h->control = mode;
     return QS_OK;
 }
 

@@ -59,7 +59,7 @@ class QuadSwarmEngine:
                  collision_hitbox_radius=2.0, collision_falloff_radius=4.0, sense_noise='default',
                  approch_goal_metric=0.5, rew_coeff=None, seed=0, device=0, env_id_offset=0,
                  device_scenario=None, quad_arm=0.0, init_random_state=False, init_vel_max=1.0, init_omega_max=2 * math.pi,
-                 use_numba=True):
+                 use_numba=True, raw_control=True, raw_control_zero_middle=True):
         if not torch.cuda.is_available():
             raise RuntimeError("QuadSwarmEngine needs a CUDA device (the env step has no CPU path)")
         self.lib = L.load()
@@ -111,6 +111,13 @@ class QuadSwarmEngine:
         self.use_numba = bool(use_numba)
         if not self.use_numba:
             L.check(self.lib.qs_set_numpy_dynamics(h, 1))
+        # QuadrotorSingle(raw_control, raw_control_zero_middle) (quadrotor_single.py:259-273): RawControl with actions in
+        # [-1, 1] (the default) or [0, 1], or the NonlinearPositionController, which ignores the actions
+        self.raw_control, self.raw_control_zero_middle = bool(raw_control), bool(raw_control_zero_middle)
+        if not self.raw_control:
+            L.check(self.lib.qs_set_control(h, L.QS_CONTROL_POSITION))
+        elif not self.raw_control_zero_middle:
+            L.check(self.lib.qs_set_control(h, L.QS_CONTROL_RAW_UNIT))
         self.D = self.lib.qs_obs_dim(h)
         self.M = self.lib.qs_num_obstacles(h)
         self.ep_len = self.lib.qs_ep_len(h)

@@ -88,8 +88,6 @@ class _EnvBase:
         from .quad_models import SAMPLERS
         if isinstance(dynamics_params, str) and dynamics_params not in SAMPLERS:
             raise AttributeError(f"module 'quadrotor_randomization' has no attribute {dynamics_params!r}")     # getattr(quad_rand, name)
-        if not (raw_control and raw_control_zero_middle):
-            raise NotImplementedError("only RawControl with zero_action_middle is supported")
         if quads_render:
             raise NotImplementedError("rendering is out of scope")
         resolve_sense_noise(sense_noise)                     # 'default', None or a dict of SensorNoise parameters
@@ -100,6 +98,9 @@ class _EnvBase:
         self.quads_view_mode = quads_view_mode
         self.quads_mode = quads_mode
         self.use_numba = use_numba                          # False: the physics of the reference's numpy path (floor model)
+        # RawControl with actions in [-1, 1] / [0, 1], or (raw_control=False) the NonlinearPositionController, which flies
+        # every drone to its goal and ignores the actions (quadrotor_single.py:259-273)
+        self.raw_control, self.raw_control_zero_middle = bool(raw_control), bool(raw_control_zero_middle)
         self.use_obstacles = bool(use_obstacles)
         self.use_downwash = bool(use_downwash)
         self.use_replay_buffer = use_replay_buffer
@@ -159,7 +160,8 @@ class _EnvBase:
             ep_time=ep_time, collision_hitbox_radius=collision_hitbox_radius,
             collision_falloff_radius=collision_falloff_radius, sense_noise=sense_noise, rew_coeff=rew_coeff,
             seed=seed, device=device, env_id_offset=env_id_offset, device_scenario=device_scenario, quad_arm=quad_arm,
-            init_random_state=init_random_state, use_numba=bool(use_numba),
+            init_random_state=init_random_state, use_numba=bool(use_numba), raw_control=self.raw_control,
+            raw_control_zero_middle=self.raw_control_zero_middle,
             # scenario.approch_goal_metric (o_base.py:16: 1.0 for the goal-sharing obstacle scenarios, else 0.5); with the
             # host-side `mix` over obstacle scenarios the value of o_random is used for every episode
             approch_goal_metric=1.0 if quads_mode in ('o_static_same_goal', 'o_dynamic_same_goal', 'o_swap_goals',
@@ -177,7 +179,10 @@ class _EnvBase:
         self.ep_len = self.engine.ep_len
         self.num_obstacles = self.engine.M
         self.observation_space = make_observation_space(obs_repr, k_eff, self.use_obstacles, room_dims)
-        self.action_space = make_action_space()
+        # envs[0]'s action space (quadrotor_multi.py): the position controller's bounds depend on its model's thrust_to_weight
+        from .quad_models import crazyflie_params
+        t2w = (crazyflie_params() if self._dyn_sources is None else self._dyn_sources[0].params)['motor']['thrust_to_weight']
+        self.action_space = make_action_space(self.raw_control, self.raw_control_zero_middle, t2w)
         assert self.observation_space.shape[0] == self.engine.D == obs_self_size + 6 * k_eff + (9 if self.use_obstacles else 0)
         # host-side episode generators: the scenario of the current episode and of the next one, per env
         mk = lambda: create_scenario(quads_mode, num_agents, room_dims=room_dims, rng=self._host_rng, ep_time=ep_time,
@@ -477,7 +482,8 @@ class QuadrotorEnvMultiBatched(_EnvBase):
                  obst_spawn_area=(8.0, 8.0), use_downwash=False, quads_mode='static_same_goal',
                  room_dims=(10., 10., 10.), sense_noise='default', device=0, seed=None, env_id_offset=0,
                  device_scenarios=True, dynamics_params='Crazyflie', dynamics_randomize_every=None, dynamics_change=None,
-                 dyn_sampler_1=None, init_random_state=False, use_numba=True):
+                 dyn_sampler_1=None, init_random_state=False, use_numba=True, raw_control=True,
+                 raw_control_zero_middle=True):
         # device-side generators (no host work per episode or per tick): o_random with obstacles, the goal-formation
         # family and mix without; every other mode uses host tables
         dev_scn = None
@@ -488,7 +494,7 @@ class QuadrotorEnvMultiBatched(_EnvBase):
         super().__init__(num_envs, num_agents, ep_time, rew_coeff, obs_repr, neighbor_visible_num, neighbor_obs_type,
                          collision_hitbox_radius, collision_falloff_radius, use_obstacles, obst_density, obst_size,
                          obst_spawn_area, use_downwash, use_numba, quads_mode, room_dims, False, ['topdown'], False,
-                         dynamics_params, True, True, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise,
+                         dynamics_params, raw_control, raw_control_zero_middle, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise,
                          init_random_state, device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn)
         self.num_agents = num_envs * num_agents
         self._truncated = torch.zeros(self.num_agents, dtype=torch.bool, device=self.engine.device)

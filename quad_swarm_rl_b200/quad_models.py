@@ -336,4 +336,5 @@ class DynamicsSource:
         return p
 
     def sample_row(self):
-        return constants_row(self.sample())
+        self.params = self.sample()          # the parameter set of the row (its thrust_to_weight bounds the controller's actions)
+        return constants_row(self.params)

@@ -55,6 +55,14 @@ def make_observation_space(obs_repr, num_use_neighbor_obs, use_obstacles, room_d
     return Box(low, high, dtype=np.float32)
 
 
-def make_action_space():
-    """RawControl.action_space with zero_action_middle (quadrotor_control.py:37-49)."""
+def make_action_space(raw_control=True, raw_control_zero_middle=True, thrust_to_weight=None):
+    """The controller's action_space (quadrotor_single.py:259-273): RawControl with zero_action_middle [-1, 1], without it
+    [0, 1] (quadrotor_control.py:37-49); NonlinearPositionController (raw_control=False) the bounds of its unused action,
+    (-1, -10 pi, -10 pi, -2 pi) .. (thrust_to_weight - 1, 10 pi, 10 pi, 2 pi) of the drone's model (:482-490)."""
+    if not raw_control:
+        max_rp, max_yaw = 5 * 2 * np.pi, 2 * np.pi
+        return Box(np.array([-1.0, -max_rp, -max_rp, -max_yaw]),
+                   np.array([thrust_to_weight - 1.0, max_rp, max_rp, max_yaw]), dtype=np.float32)
+    if not raw_control_zero_middle:
+        return Box(np.zeros(4), np.ones(4), dtype=np.float32)
     return Box(-np.ones(4), np.ones(4), dtype=np.float32)

@@ -1,6 +1,7 @@
 """Small workload for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): both step-kernel shapes, both
 launch-chaining modes, resets, contacts, every device-side scenario id, rollout, state and statistics kernels, the
-pre-generated episode records, per-drone dynamics, obstacle randomisation and the training-wrapper kernel (replay on), and the courier-warp hand-over of balanced grids."""
+pre-generated episode records, per-drone dynamics, obstacle randomisation and the training-wrapper kernel (replay on), the courier-warp hand-over of balanced grids, and the step kernels of the
+control modes (position controller, [0, 1] actions) on both dynamics paths."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -69,4 +70,9 @@ os.environ.pop('QS_PDL', None)                       # default launch rule: bala
 run(OBST, 600, 'o_random', steps=8)
 run(dict(num_agents=8, neighbor_visible_num=6), 600, 'swap_goals', steps=8)
 run_extras(E=600, steps=30, chained=True, dynamics=False)      # wrapped control steps, block-chained with the wrapper kernel
+# the control modes of qs_set_control on both dynamics paths (qs_step_pc.cu, qs_step_pc_npy.cu)
+for ctl in (dict(raw_control=False), dict(raw_control_zero_middle=False)):
+    for use_numba in (True, False):
+        run(dict(OBST, use_numba=use_numba, **ctl), 13, 'o_random', steps=10)
+        run(dict(num_agents=8, neighbor_visible_num=6, use_numba=use_numba, **ctl), 600, 'swap_goals', steps=8)
 print('sanitize workload done')
