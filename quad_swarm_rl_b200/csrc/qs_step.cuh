@@ -624,10 +624,12 @@ __device__ __forceinline__ void hand_load(const float* hand, int lane, Agent& s,
 // bias (p.gyro_bias, when that model is on) rides in registers across the steps of a launch.  Same shape as DYN.
 // qs_step_npy.cu compiles this kernel once more, as qs_step_kernel_npy, with the floor model of the reference's numpy path
 // (QS_NUMPY_DYNAMICS, qs_set_numpy_dynamics).  qs_step_pc.cu / qs_step_pc_npy.cu compile it as qs_step_kernel_pc /
-// qs_step_kernel_pc_npy with the control modes of qs_set_control (QS_CONTROL_MODES).
+// qs_step_kernel_pc_npy with the control modes of qs_set_control (QS_CONTROL_MODES; same shape as DYN).
 template <int NP, bool SPLIT, bool SCN, bool HO, bool DYN = false, bool NZ = false>
 __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>()) qs_step_kernel(const __grid_constant__ StepParams p) {
-    static_assert(!NZ || (!SPLIT && !HO), "the custom sensor-noise model runs in the single-warp shape with the grid-wide wait");
+    static_assert(!(DYN || NZ || QS_CONTROL_MODES) || (!SPLIT && !HO),
+                  "per-drone constants, the custom sensor-noise model and the control modes run in the single-warp shape with "
+                  "the grid-wide wait");
     extern __shared__ __align__(128) float2 s_obst[];
     __shared__ int s_late;          // courier launches: a block with a goal event behind the observation is released at its end
     __shared__ unsigned long long s_rows;      // courier launches: mbarrier, completes when the previous instance's observation rows are out

@@ -421,18 +421,15 @@ static int dispatch_np(int NP, F&& f) {
 
 #include "qs_step_select.cuh"
 
-// The numpy dynamics path's step kernels (qs_step_npy.cu): the same shapes, selected by the same rule.
-namespace qs_npy {
-void* step_kernel_npy(int NP, bool split, bool scn, bool ho, bool dyn, bool nz);
-}
-// The step kernels of the control modes of qs_set_control (qs_step_pc.cu, qs_step_pc_npy.cu): single-warp shape with the
-// grid-wide wait only.
-namespace qs_pc {
-void* step_kernel_pc(int NP, bool scn, bool dyn, bool nz);
-}
-namespace qs_pc_npy {
-void* step_kernel_pc(int NP, bool scn, bool dyn, bool nz);
-}
+// The step kernels of the other translation units, each with its select_step_kernel (qs_step_select.cuh): the numpy
+// dynamics path (qs_step_npy.cu) and the control modes of qs_set_control on either path (qs_step_pc.cu, qs_step_pc_npy.cu).
+namespace qs_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+namespace qs_pc { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+namespace qs_pc_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+
+// [control mode other than QS_CONTROL_RAW][numpy dynamics path]
+static void* (*const select_step_kernel_of[2][2])(int, bool, bool, bool, bool, bool) = {
+    {qs::select_step_kernel, qs_npy::select_step_kernel}, {qs_pc::select_step_kernel, qs_pc_npy::select_step_kernel}};
 
 struct StepShape {
     KernelFn fn;
@@ -483,31 +480,28 @@ static int courier_workers(QsHandle* h, KernelFn fn, int wpc_even) {
 //    where that lets an SM hold a CTA of the next step beside those of this one (courier_workers): c3 / c5 run 256 CTAs of
 //    4 workers + courier (160 threads, up to three per SM) instead of 128 CTAs of 8 + 1.
 //  * otherwise: 64-thread single-warp CTAs over as many waves as it takes.
-// Host logic only; the CUDA calls are the occupancy queries of a handle's first hand-over and courier decisions, whose
-// errors it returns.
+// DYN, NZ and the control modes run in the single-warp shape with the grid-wide wait only; the kernel comes from the
+// select_step_kernel of the handle's control mode and dynamics path.  Host logic only; the CUDA calls are the occupancy
+// queries of a handle's first hand-over and courier decisions, whose errors it returns.
 static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const int NP = h->NP, sms = h->sms;
     const bool dyn = h->st.dyn != nullptr, nz = h->nz_on;
-    const bool ctl = h->control != QS_CONTROL_RAW;          // qs_set_control: like dyn / nz, single-warp shape, grid-wide wait
+    const bool ctl = h->control != QS_CONTROL_RAW;          // qs_set_control
+    const bool grid_wait_only = dyn || nz || ctl;           // only the single-warp kernels with the grid-wide wait exist
     const long long phys_warps = ((long long)h->cfg.num_envs * NP + 31) / 32;
     int wpc = (int)((phys_warps + sms - 1) / sms);          // worker warps per CTA of a balanced grid
     const bool balance_fits = NP < 16 && wpc >= 2 && wpc * 32 <= QS_LB && (wpc * 32) % NP == 0;
     const bool courier_fits = balance_fits && (wpc + 1) * 32 <= QS_LB;
-    const bool courier_shape = h->chained && !dyn && !nz && !ctl && courier_fits;
+    const bool courier_shape = h->chained && !grid_wait_only && courier_fits;
     const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
-    s.split = want_split && p.obs_stage && NP > 1 && !dyn && !nz && !ctl && !h->obst_random;
+    s.split = want_split && p.obs_stage && NP > 1 && !grid_wait_only && !h->obst_random;
     const bool balanced = !s.split && balance_fits;
     const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
     const bool scn = p.use_obst ? ticked_obst
                                 : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
                                    p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
-    auto kernel = [&](bool ho, bool k_dyn, bool k_nz) {
-        KernelFn fn = nullptr;
-        if (ctl) return (KernelFn)(h->numpy_dyn ? qs_pc_npy::step_kernel_pc(NP, scn, k_dyn, k_nz) : qs_pc::step_kernel_pc(NP, scn, k_dyn, k_nz));
-        if (h->numpy_dyn) return (KernelFn)qs_npy::step_kernel_npy(NP, s.split, scn, ho, k_dyn, k_nz);      // qs_set_numpy_dynamics
-        dispatch_np(NP, [&](auto np) { fn = step_kernel<decltype(np)::value>(s.split, scn, ho, k_dyn, k_nz); return QS_OK; });
-        return fn;
-    };
+    const auto select = select_step_kernel_of[ctl][h->numpy_dyn ? 1 : 0];     // qs_set_control, qs_set_numpy_dynamics
+    auto kernel = [&](bool ho, bool k_dyn, bool k_nz) { return (KernelFn)select(NP, s.split, scn, ho, k_dyn, k_nz); };
     // A balanced grid that will carry the courier warp (the hand-over is, or will be, chosen below): its worker warps per CTA
     // come from the kernel's occupancy (courier_workers), and the env -> block mapping follows them.
     if (balanced && courier_shape && h->handover != 0) {
@@ -549,7 +543,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     if (balanced && s.smem < pad) s.smem = pad;
     // The hand-over kernels pay off only between step grids that follow each other directly; an unchained handle uses the
     // grid-wide wait (formally safe after any predecessor) and never pre-fetches across the dependency wait.
-    s.ho = h->handover == 1 && h->chained && !dyn && !nz && !ctl;
+    s.ho = h->handover == 1 && h->chained && !grid_wait_only;
     s.fn = kernel(s.ho, dyn, nz);
     return QS_OK;
 }
@@ -628,11 +622,9 @@ static int launch_reset(QsHandle* h, const StepParams& p, cudaStream_t s) {
     const size_t smem = h->cfg.use_obstacles ? (size_t)envs_per_block * h->M * sizeof(float2) : 0;
     int rc = dispatch_np(h->NP, [&](auto np) {
         constexpr int NPv = decltype(np)::value;
-        if (h->init_random) {
-            if (h->nz_on) qs_reset_kernel<NPv, true, true><<<grid, kBlock, smem, s>>>(p);
-            else qs_reset_kernel<NPv, false, true><<<grid, kBlock, smem, s>>>(p);
-        } else if (h->nz_on) qs_reset_kernel<NPv, true><<<grid, kBlock, smem, s>>>(p);
-        else qs_reset_kernel<NPv><<<grid, kBlock, smem, s>>>(p);
+        const auto fn = h->init_random ? (h->nz_on ? qs_reset_kernel<NPv, true, true> : qs_reset_kernel<NPv, false, true>)
+                                       : (h->nz_on ? qs_reset_kernel<NPv, true, false> : qs_reset_kernel<NPv, false, false>);
+        fn<<<grid, kBlock, smem, s>>>(p);
         return QS_OK;
     });
     if (rc != QS_OK) return rc;

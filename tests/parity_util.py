@@ -4,8 +4,16 @@
 The oracle is float64, the kernels float32.  Trajectories are teacher-forced: every `resync` steps (and after
 any step whose discrete decisions sat closer to their thresholds than float32 can resolve) the oracle's state is
 written into the engine with qs_set_state, so the comparison measures per-step error, not chaotic divergence.
+
+Also the resource usage of the built library's kernels (kernel_resources), which the CPU tests check.
 """
+import os
+import re
+import shutil
+import subprocess
+
 import numpy as np
+import pytest
 import torch
 
 from oracle import quadswarm_oracle as qo
@@ -372,3 +380,22 @@ def run_parity(pair, T, rs, resync=20, rtol=1e-4, atol=1e-4, action_scale=1.0, c
         if need_sync:
             pair.sync_device_from_oracle()
     return rep
+
+
+def kernel_resources(pattern):
+    """Registers, stack frame and local memory of the built library's kernels (`cuobjdump --dump-resource-usage`):
+    {key: {'REG': n, 'STACK': n, 'LOCAL': n}} for every function whose mangled name matches the regex `pattern`, keyed by
+    the match's groups, digit groups as ints.  Skips the test when cuobjdump or the library is not there."""
+    tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
+    if not (os.path.exists(tool) and os.path.exists(L.LIB_PATH)):
+        pytest.skip('cuobjdump or the library not available')
+    out = subprocess.run([tool, '--dump-resource-usage', L.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    usage, key = {}, None
+    for line in out.splitlines():
+        if 'Function' in line:
+            m = re.search(pattern, line)
+            key = tuple(int(g) if g and g.isdigit() else g for g in m.groups()) if m else None
+        elif key is not None and 'REG:' in line:
+            usage[key] = {k: int(v) for k, v in re.findall(r'(REG|STACK|LOCAL):(\d+)', line)}
+            key = None
+    return usage

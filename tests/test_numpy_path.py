@@ -163,21 +163,8 @@ def test_entry_point_rejects_a_null_handle_without_gpu():
 def test_numpy_path_kernels_fit_like_the_default_ones():
     """The numpy path has its own step kernels, one per default instantiation, built from the same body; the ones that can
     carry the courier warp keep its budget (<= 128 registers, no local memory: two CTAs of consecutive steps per SM)."""
-    import shutil
-    import subprocess
-    lib = os.environ.get('QS_LIB') or os.path.join(ROOT, 'quad_swarm_rl_b200', 'libquadswarm.so')
-    tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
-    if not (os.path.exists(tool) and os.path.exists(lib)):
-        pytest.skip('cuobjdump or the library not available')
-    out = subprocess.run([tool, '--dump-resource-usage', lib], capture_output=True, text=True, check=True).stdout
-    usage, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r'qs_step_kernel(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE', line) if 'Function' in line else None
-        if m:
-            name = (bool(m.group(1)),) + tuple(int(x) for x in m.groups()[1:])
-        elif name is not None and 'REG:' in line:
-            usage[name] = {k: int(v) for k, v in re.findall(r'(REG|STACK|LOCAL):(\d+)', line)}
-            name = None
+    from tests.parity_util import kernel_resources
+    usage = kernel_resources(r'qs_step_kernel(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE')
     default = sorted(k[1:] for k in usage if not k[0])
     assert len(default) == 84 and sorted(k[1:] for k in usage if k[0]) == default
     courier = {k: v for k, v in usage.items() if k[0] and k[1] < 16 and k[2:] == (0, 0, 1, 0, 0)}

@@ -208,31 +208,13 @@ def test_entry_point_rejects_a_null_handle_without_gpu():
     assert lib.qs_set_control(None, 2) == -1 and b'null' in lib.qs_last_error()
 
 
-def _resource_usage():
-    import shutil
-    import subprocess
-    lib = os.environ.get('QS_LIB') or os.path.join(ROOT, 'quad_swarm_rl_b200', 'libquadswarm.so')
-    tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
-    if not (os.path.exists(tool) and os.path.exists(lib)):
-        pytest.skip('cuobjdump or the library not available')
-    out = subprocess.run([tool, '--dump-resource-usage', lib], capture_output=True, text=True, check=True).stdout
-    usage, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r'qs_step_kernel_pc(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE', line) if 'Function' in line else None
-        if m:
-            name = (bool(m.group(1)),) + tuple(int(x) for x in m.groups()[1:])
-        elif name is not None and 'REG:' in line:
-            usage[name] = {k: int(v) for k, v in re.findall(r'(REG|STACK|LOCAL):(\d+)', line)}
-            name = None
-    return usage
-
-
 def test_control_kernels_instantiate_the_grid_wide_wait_shape_only():
     """Per dynamics path: NP in {1, ..., 32} x SCN x DYN x NZ, never the split or hand-over shapes; no local memory beyond
     the stack frame."""
-    usage = _resource_usage()
+    from tests.parity_util import kernel_resources
+    usage = kernel_resources(r'qs_step_kernel_pc(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE')
     for npy in (False, True):
-        keys = sorted(k[1:] for k in usage if k[0] is npy)
+        keys = sorted(k[1:] for k in usage if bool(k[0]) is npy)
         assert keys == sorted((NP, 0, scn, 0, dyn, nz) for NP in (1, 2, 4, 8, 16, 32) for scn in (0, 1)
                               for dyn in (0, 1) for nz in (0, 1))
     for k, v in usage.items():

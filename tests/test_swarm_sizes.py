@@ -11,20 +11,18 @@ there), asserts a minimum number of compared env-steps, and asserts that its eve
 and pillar contacts, goal events) actually happened.
 
 CPU: every step-kernel instantiation NP = 16 / 32 can select is in the library and uses no local memory."""
-import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
-from tests.parity_util import DevicePair, Pair, SampledPair, run_parity
+from tests.parity_util import DevicePair, Pair, SampledPair, kernel_resources, run_parity
 from tests.test_gpu_parity import _cluster_hook, _dyn_rows, _obst_hook, _params_of, _room_hook
 from tests.test_init_random_state import _arm_oracles, _on
 from tests.test_numpy_path import _plant_floor
 from tests.test_sensor_noise import _noise_pair
-from tests.test_step_shape import LIB, ROOT, _stagger
+from tests.test_step_shape import ROOT, _stagger
 
 FLOOR = 'xyz_vxyz_R_omega_floor'
 WALL = 'xyz_vxyz_R_omega_wall'
@@ -734,32 +732,12 @@ def test_replay_stores_collisions_of_high_lanes(n, pair_ids):
 # ---------------------------------------------------------------------------------------------------------------------
 # 8. CPU: the NP = 16 / 32 instantiations in the built library
 # ---------------------------------------------------------------------------------------------------------------------
-STEP = re.compile(r'qs_step_kernel(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE')
-OTHER = re.compile(r'(qs_reset_kernel|qs_pregen_kernel|qs_wrap_kernel)ILi(16|32)E(\w*?)EEvN')
-
-
 def _usage():
     """Resource usage of the step kernels {(path, NP, SPLIT, SCN, HO, DYN, NZ): {REG, STACK, LOCAL}} and of the NP = 16 / 32
     reset, pre-generation and wrapper kernels {(name, NP, other template arguments): ...} in the built library."""
-    tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
-    if not os.path.exists(tool):
-        pytest.skip('cuobjdump not available')
-    if not os.path.exists(LIB):
-        pytest.skip('library not built')
-    out = subprocess.run([tool, '--dump-resource-usage', LIB], capture_output=True, text=True, check=True).stdout
-    steps, other, slot = {}, {}, None
-    for line in out.splitlines():
-        if 'Function' in line:
-            m, m2 = STEP.search(line), OTHER.search(line)
-            slot = None
-            if m:
-                slot = steps, ('npy' if m.group(1) else 'default',) + tuple(int(x) for x in m.groups()[1:])
-            elif m2:
-                slot = other, (m2.group(1), int(m2.group(2)), m2.group(3))
-        elif slot is not None and 'REG:' in line:
-            slot[0][slot[1]] = {k: int(v) for k, v in re.findall(r'(REG|STACK|LOCAL):(\d+)', line)}
-            slot = None
-    return steps, other
+    steps = kernel_resources(r'qs_step_kernel(_npy)?ILi(\d+)ELb([01])ELb([01])ELb([01])ELb([01])ELb([01])EE')
+    other = kernel_resources(r'(qs_reset_kernel|qs_pregen_kernel|qs_wrap_kernel)ILi(16|32)E(\w*?)EEvN')
+    return {('npy' if k[0] else 'default',) + k[1:]: v for k, v in steps.items()}, other
 
 
 def test_np16_np32_step_instantiations_present_without_local_memory():
