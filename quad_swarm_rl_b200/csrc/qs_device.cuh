@@ -593,9 +593,11 @@ __device__ __forceinline__ void physics_substep(Agent& s, const float cmd[4], bo
                     fx = mag; fy = 0.f;
                 }
             } else {
-                // sliding: friction against the horizontal velocity direction; atan2(0, 0) = 0 -> direction (1, 0)
+                // sliding: friction against the horizontal velocity direction.  With no horizontal velocity atan2(vy, vx)
+                // sees signed zeros: atan2(+-0, +0) = +-0 -> direction (1, 0), atan2(+-0, -0) = +-pi -> (-1, 0) (the
+                // sin(+-pi) = +-1.2e-16 is dropped)
                 const float h2 = s.vel[0] * s.vel[0] + s.vel[1] * s.vel[1];
-                float ca = 1.f, sa = 0.f;
+                float ca = copysignf(1.f, s.vel[0]), sa = 0.f;
                 if (h2 > 0.f) {
                     const float inv = frsqrt(h2);
                     ca = s.vel[0] * inv; sa = s.vel[1] * inv;
