@@ -244,6 +244,66 @@ int qs_set_state(QsHandle* h, const uint8_t* env_mask_dev, const float* agent_f3
 #define QS_DYN_ROW 40
 int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const float* rows_dev, int at_next_reset, void* stream);
 
+/* Dynamics randomisation on the device — replaces the dynamics_params / dynamics_change / dyn_sampler_1 / dyn_sampler_2 /
+ * dynamics_randomize_every pipeline of QuadrotorSingle (quadrotor_single.py:186-211,359-390; quadrotor_randomization.py).
+ * Every drone's row is sampled on the device, in float64, and rounded to float32 once: base set (a fixed parameter tree or
+ * RandomQuad, quadrotor_randomization.py:142-243) -> dynamics_change -> sampler 1 -> sampler 2 -> check_quad_param_limits ->
+ * the link inertia model and the derived constants of qs_set_dynamics' row.  The row of drone i of env e in episode k is a
+ * function of (seed, env_id_offset + e, k, i) only (draw site 24, episode-keyed): k = 0 is the construction sample, an
+ * (auto-)reset that starts episode k >= 1 resamples when randomize_every > 0 and k % randomize_every == 0 (the reference's
+ * (traj_count + 1) % every == 0 with traj_count = k - 1), and the drone keeps its row otherwise.
+ *
+ * The parameter tree is a flat vector of QS_DYN_LEAVES leaves, each a presence flag plus a float64 value; array leaves are
+ * one leaf per element.  Leaf ids (QS_DL_*) name the tree's paths; `order` lists the present leaves in the order the tree
+ * is walked (dict order of the host pipeline), which is the order RelativeSampler draws in. */
+enum {
+    QS_DL_BODY_L = 0, QS_DL_BODY_W, QS_DL_BODY_H, QS_DL_BODY_M, QS_DL_BODY_DENSITY,                          /* geom.body */
+    QS_DL_PAYLOAD_L, QS_DL_PAYLOAD_W, QS_DL_PAYLOAD_H, QS_DL_PAYLOAD_M, QS_DL_PAYLOAD_DENSITY,                /* geom.payload */
+    QS_DL_ARMS_L, QS_DL_ARMS_W, QS_DL_ARMS_H, QS_DL_ARMS_M, QS_DL_ARMS_DENSITY,                              /* geom.arms */
+    QS_DL_MOTORS_H, QS_DL_MOTORS_R, QS_DL_MOTORS_M, QS_DL_MOTORS_DENSITY,                                    /* geom.motors */
+    QS_DL_PROPS_H, QS_DL_PROPS_R, QS_DL_PROPS_M, QS_DL_PROPS_DENSITY,                                        /* geom.propellers */
+    QS_DL_MOTOR_POS_X, QS_DL_MOTOR_POS_Y, QS_DL_MOTOR_POS_Z,                                                 /* geom.motor_pos.xyz */
+    QS_DL_ARMS_ANGLE, QS_DL_ARMS_Z,                                                                          /* geom.arms_pos */
+    QS_DL_PAYLOAD_X, QS_DL_PAYLOAD_Y, QS_DL_PAYLOAD_Z_SIGN,                                                  /* geom.payload_pos */
+    QS_DL_DAMP_VEL, QS_DL_DAMP_OMEGA_QUADRATIC,                                                              /* damp */
+    QS_DL_THRUST_NOISE_RATIO,                                                                                /* noise */
+    QS_DL_THRUST_TO_WEIGHT, QS_DL_ASSYMETRY0, QS_DL_ASSYMETRY1, QS_DL_ASSYMETRY2, QS_DL_ASSYMETRY3,         /* motor */
+    QS_DL_TORQUE_TO_THRUST, QS_DL_LINEARITY, QS_DL_C_DRAG, QS_DL_C_ROLL, QS_DL_DAMP_TIME_UP, QS_DL_DAMP_TIME_DOWN,
+    QS_DYN_LEAVES
+};
+typedef struct QsDynLeaves {
+    double value[QS_DYN_LEAVES];
+    uint8_t present[QS_DYN_LEAVES];
+    uint8_t reserved_[3];
+} QsDynLeaves;
+#define QS_DYN_BASE_FIXED 0             /* `params` is the base set (Crazyflie, DefaultQuad, MediumQuad, a dict) */
+#define QS_DYN_BASE_RANDOM_QUAD 1       /* RandomQuad: 31 draws; `params.present` is its tree (values unused) */
+#define QS_DYN_SAMPLER_NONE 0
+#define QS_DYN_SAMPLER_RELATIVE_NORMAL 1    /* RelativeSampler(sampler='normal'): value ~ N(v, (ratio / 2 |v|)^2), one draw per leaf */
+#define QS_DYN_SAMPLER_RELATIVE_UNIFORM 2   /* RelativeSampler(sampler='uniform'): value ~ U(v - v ratio, v + v ratio) */
+#define QS_DYN_SAMPLER_CONST 3              /* ConstValueSampler: every present leaf of `samp` replaces the tree's value */
+typedef struct QsDynSampler {
+    int32_t base;                   /* QS_DYN_BASE_* */
+    int32_t sampler[2];             /* QS_DYN_SAMPLER_* of dyn_sampler_1, dyn_sampler_2 */
+    int32_t n_order;
+    int32_t order[QS_DYN_LEAVES];   /* the present leaves of the tree in walk order (n_order of them) */
+    QsDynLeaves params;             /* the tree: which leaves exist, and for QS_DYN_BASE_FIXED their values */
+    QsDynLeaves change;             /* dynamics_change: present leaves override the base set's values */
+    QsDynLeaves samp[2];            /* relative samplers: the noise ratio of every leaf of the tree; const: the new values */
+} QsDynSampler;
+/* Call after qs_create and before the first qs_reset / qs_step: allocates the per-drone tables and writes every drone's
+ * construction sample.  randomize_every = 0 is the reference's None (the construction sample only).  Later calls, a handle
+ * that already has rows from qs_set_dynamics, malformed specs (unknown kinds, leaves outside the tree, missing leaves the
+ * model needs) and non-finite values fail with QS_ERR_INVALID_ARG.  qs_set_dynamics fails on such a handle: the sampler owns
+ * the rows.  The sampling runs ahead of the resets where it can (beside the next-episode generator, before an explicit
+ * reset) and otherwise right behind the step grid whose reset needs the row, with the same results.  A sampler handle
+ * steps with DYN kernels of its own (single-warp shape, grid-wide wait), one control step per grid: its qs_rollout launches
+ * num_steps grids. */
+int qs_set_dynamics_sampler(QsHandle* h, const QsDynSampler* spec_host, int randomize_every);
+/* The live rows of every drone, rows_dev [E,N,QS_DYN_ROW] floats (device -> device copy on `stream`).  Fails on a handle
+ * without per-drone rows (neither qs_set_dynamics nor qs_set_dynamics_sampler was called). */
+int qs_get_dynamics(QsHandle* h, float* rows_dev, void* stream);
+
 /* Per-episode pillar density / size randomisation — replaces ExperienceReplayWrapper's domain randomisation
  * (gym_art/quadrotor_multi/quad_experience_replay.py:76-88,108-118,196-205: np.random.choice over np.arange(min, max, step))
  * and QuadrotorEnvMulti.reset(obst_density, obst_size) (quadrotor_multi.py:339-351).  densities_host [n_densities] and

@@ -19,6 +19,7 @@ QS_STATE_U32 = 4
 QS_STATE_ENV_I32 = 36
 QS_MAX_AGENTS = 32
 QS_DYN_ROW = 40
+QS_DYN_LEAVES = 45
 QS_CONTROL_RAW, QS_CONTROL_RAW_UNIT, QS_CONTROL_POSITION = 0, 1, 2
 SCENARIO_HOST_TABLES, SCENARIO_O_RANDOM = 0, 1
 # scenarios with a device-side generator (QS_SCENARIO_* of include/quadswarm.h), by their reference names
@@ -67,6 +68,43 @@ class QsWrapConfig(C.Structure):
                 ('replay_always_active', C.c_int32), ('reserved_', C.c_int32 * 4)]
 
 
+class QsDynLeaves(C.Structure):
+    _fields_ = [('value', C.c_double * QS_DYN_LEAVES), ('present', C.c_uint8 * QS_DYN_LEAVES), ('reserved_', C.c_uint8 * 3)]
+
+
+class QsDynSampler(C.Structure):
+    _fields_ = [('base', C.c_int32), ('sampler', C.c_int32 * 2), ('n_order', C.c_int32), ('order', C.c_int32 * QS_DYN_LEAVES),
+                ('params', QsDynLeaves), ('change', QsDynLeaves), ('samp', QsDynLeaves * 2)]
+
+
+def _leaves(present_value):
+    out = QsDynLeaves()
+    present, value = present_value
+    out.present[:] = [int(x) for x in present]
+    out.value[:] = [float(x) for x in value]
+    return out
+
+
+def dyn_sampler_struct(spec):
+    """quad_models.dynamics_sampler_spec(...) -> QsDynSampler."""
+    out = QsDynSampler()
+    out.base = int(spec['base'])
+    out.sampler[:] = [int(k) for k in spec['sampler']]
+    out.n_order = len(spec['order'])
+    out.order[:len(spec['order'])] = [int(k) for k in spec['order']]
+    out.params, out.change = _leaves(spec['params']), _leaves(spec['change'])
+    out.samp[0], out.samp[1] = _leaves(spec['samp'][0]), _leaves(spec['samp'][1])
+    return out
+
+
+def dyn_sampler_spec_of(st):
+    """QsDynSampler -> the spec dict of quad_models.dynamics_sampler_spec."""
+    import numpy as np
+    leaves = lambda l: (np.array(l.present[:], np.uint8), np.array(l.value[:], np.float64))
+    return dict(base=st.base, order=np.array(st.order[:st.n_order], np.int32), params=leaves(st.params), change=leaves(st.change),
+                sampler=list(st.sampler), samp=[leaves(st.samp[0]), leaves(st.samp[1])])
+
+
 QS_WRAP_AGG = 149
 WA = dict(AGENT_EPISODES=0, TRUE_REWARD=1, RAW0=2, REW0=10, ACT_MEAN0=18, ACT_STD0=22, ENV_EPISODES=26, ENV_STAT0=27, DIST0=38,
           SUCCESS=41, DEADLOCK=42, COL=43, NEIGHBOR_COL=44, OBST_COL=45, REPLAY_ENV_EPISODES=46, REPLAY_COLLISIONS=47,
@@ -98,6 +136,8 @@ EXPORTS = {
     'qs_set_chained': (C.c_int, [C.c_void_p, C.c_int]),
     'qs_set_obstacle_randomization': (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_float), C.c_int]),
     'qs_set_dynamics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    'qs_set_dynamics_sampler': (C.c_int, [C.c_void_p, C.POINTER(QsDynSampler), C.c_int]),
+    'qs_get_dynamics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_sensor_noise': (C.c_int, [C.c_void_p, C.POINTER(QsSensorNoise)]),
     'qs_get_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_gyro_bias': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

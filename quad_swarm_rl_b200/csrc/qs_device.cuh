@@ -49,6 +49,11 @@ constexpr float FLOOR_THRESHOLD_NP = 0.05f;       // floor threshold and snap he
 #ifndef QS_CONTROL_MODES
 #define QS_CONTROL_MODES 0
 #endif
+// QS_DYN_SAMPLER = 1 (set by the qs_step_ds*.cu units only): the DYN step kernels of handles with the device-side dynamics
+// sampler (qs_set_dynamics_sampler; the sampler's reset path in qs_step_kernel).
+#ifndef QS_DYN_SAMPLER
+#define QS_DYN_SAMPLER 0
+#endif
 constexpr float SIM_DT = 0.005f;                  // quadrotor_single.py:157
 constexpr float CONTROL_DT = 0.01f;               // quadrotor_multi.py:83
 constexpr int SIM_STEPS = 2;                      // quadrotor_single.py:102
@@ -114,6 +119,12 @@ struct NoiseModel {
     int rot;                // quat_std or quat_range != 0: the observed rotation is perturbed
 };
 
+// qs_set_dynamics_sampler's arguments, in device memory (read only at resampling resets)
+struct DynSampler {
+    QsDynSampler spec;
+    int every;              // randomize_every: resample at the reset that starts episode g when g % every == 0; 0 = never
+};
+
 struct StepParams {
     alignas(64) unsigned char obs_map[128];     // CUtensorMap of the caller's observation array (obs_bulk == 1), see quadswarm.cu
     DevState st;
@@ -157,6 +168,9 @@ struct StepParams {
     int init_random;                    // qs_set_init_random_state: every spawn gets a random vel / omega / R (random_init_state)
     float init_vel_max, init_omega_max;
     int control;                        // qs_set_control: QS_CONTROL_*; read only by the kernels of qs_step_pc.cu
+    const DynSampler* dyn;              // qs_set_dynamics_sampler (qs_dyn_sampler.cuh), or null; read only by the DYN
+                                        // instantiations and the sampler's kernels.  It takes the last 8 bytes of the
+                                        // struct's padding: every other kernel keeps its parameter layout.
 };
 
 struct Agent {

@@ -56,6 +56,11 @@ enum Site : uint32_t {
     // Upside-down first floor contact of the numpy dynamics path (qs_set_numpy_dynamics; floor_interaction,
     // quadrotor_dynamics.py:434-437), step-keyed like SITE_FLOOR_YAW.  CPU twin: oracle/numpy_path_oracle.py.
     SITE_FLOOR_YAW_NP = 23, // (i,j) uniforms v[k], j = sub-step, k = rejection try of randyaw()
+    // Per-drone physical constants of the device-side dynamics sampler (qs_set_dynamics_sampler, qs_dyn_sampler.cuh),
+    // episode-keyed like SITE_SPAWN_U (episode 0 = the construction sample).  Draw k of drone i is block k: a uniform is
+    // low + (high - low) u01(word 0), a normal is the float64 Box-Muller n0 of words (0, 1).  CPU twin:
+    // oracle/dyn_sampler_oracle.py.
+    SITE_DYN = 24,          // (i)   block k = the k-th scalar the host pipeline draws
 };
 
 constexpr int RESET_YAW_MAX_TRIES = 64;     // also caps the SITE_FLOOR_YAW_NP loop (reference: unbounded; p(re-draw) = 2/3)

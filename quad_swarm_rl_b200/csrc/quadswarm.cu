@@ -62,6 +62,8 @@ struct QsHandle {
     float init_vel_max, init_omega_max;
     int numpy_dyn;        // qs_set_numpy_dynamics
     int control;          // qs_set_control: QS_CONTROL_*
+    DynSampler* dyn_spec; // qs_set_dynamics_sampler: device copy of the spec and its randomize_every, or null
+    int dyn_every;        // its randomize_every
     cudaStream_t last_stream;   // stream of the most recent asynchronous call of this handle
     bool async_pending;
     // staging for the *_host entry points (pinned host + device mirrors)
@@ -184,6 +186,7 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.gyro_bias = h->gyro_bias;
     p.init_random = h->init_random; p.init_vel_max = h->init_vel_max; p.init_omega_max = h->init_omega_max;
     p.control = h->control;
+    p.dyn = h->dyn_spec;
 }
 
 // Observation write-out mode of a step launch (qs_step.cuh, emit_observation_tile): the bulk-copy engine needs a 16-byte
@@ -393,6 +396,48 @@ __global__ void k_set_dynamics(DevState st, int E, int N, const uint8_t* mask, c
     if (at_next_reset && t < E && (mask == nullptr || mask[t])) st.dyn_pending[t] = 1;
 }
 
+// qs_set_dynamics_sampler: the construction sample (episode 0) of every drone into the live table
+__global__ void k_dyn_construct(const __grid_constant__ StepParams p) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)p.E * p.N) return;
+    const int env = (int)(t / p.N), i = (int)(t % p.N);
+    sample_dyn_row(p.dyn, episode_key(p, env, 0), i, p.st.dyn + t * (QS_DYN_ROW / 4));
+}
+
+// The device-side dynamics sampler around the resets.  AHEAD = false: launched behind every step grid of a sampler handle
+// that resamples; AHEAD = true: beside qs_pregen_kernel (same cadence) and before every explicit reset, on its env mask
+// (p.env_mask).
+//  * dyn_pending = -g: a step grid started episode g, which resamples, without a prepared row: sample it into the live table;
+//  * AHEAD: then, for the episode g = epi.x + 1 the env starts at its next reset: if it resamples (dyn_due) and has no prepared row
+//    yet, sample its rows into next_dyn and tag them with dyn_pending = g, which that reset latches (qs_step_kernel, DYN;
+//    qs_reset_kernel); if it does not, dyn_pending = 0, so that qs_reset_kernel latches nothing (also after the episode
+//    number was set back since a tag was written).
+// Lanes as in qs_pregen_kernel: the drones of an env sit in one warp, which reads the tag before lane 0 rewrites it.
+template <int NP, bool AHEAD>
+__global__ void __launch_bounds__(128) qs_dyn_pregen_kernel(const __grid_constant__ StepParams p) {
+    const DevState& st = p.st;
+    const int i = (threadIdx.x & 31) & (NP - 1);
+    const int env = blockIdx.x * (blockDim.x / NP) + threadIdx.x / NP;
+    const bool env_ok = env < p.E && (p.env_mask == nullptr || p.env_mask[env] != 0);
+    int g = 0, pend = 0;
+    if (env_ok) {
+        g = st.epi[env].x + 1;
+        pend = st.dyn_pending[env];
+    }
+    const long long a = (long long)env * p.N + i;
+    if (pend < 0 && i < p.N) sample_dyn_row(p.dyn, episode_key(p, env, -pend), i, st.dyn + a * (QS_DYN_ROW / 4));
+    if (!AHEAD) {               // behind a step grid: only the rows its resets did not find
+        __syncwarp();
+        if (i == 0 && pend < 0) st.dyn_pending[env] = 0;
+        return;
+    }
+    const bool due = env_ok && dyn_due(g, p.dyn->every);
+    if (due && pend != g && i < p.N) sample_dyn_row(p.dyn, episode_key(p, env, g), i, st.next_dyn + a * (QS_DYN_ROW / 4));
+    const int pend_after = due ? g : 0;
+    __syncwarp();
+    if (i == 0 && env_ok && pend != pend_after) st.dyn_pending[env] = pend_after;
+}
+
 __global__ void k_read_stats(DevState st, int E, int N, int32_t* env_stats, float* agent_stats) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t < (long long)E * N && agent_stats) {
@@ -426,10 +471,16 @@ static int dispatch_np(int NP, F&& f) {
 namespace qs_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 namespace qs_pc { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 namespace qs_pc_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+// the DYN kernels of handles with the device-side dynamics sampler (qs_step_ds*.cu)
+namespace qs_ds { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+namespace qs_ds_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+namespace qs_ds_pc { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
+namespace qs_ds_pc_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 
-// [control mode other than QS_CONTROL_RAW][numpy dynamics path]
-static void* (*const select_step_kernel_of[2][2])(int, bool, bool, bool, bool, bool) = {
-    {qs::select_step_kernel, qs_npy::select_step_kernel}, {qs_pc::select_step_kernel, qs_pc_npy::select_step_kernel}};
+// [dynamics sampler][control mode other than QS_CONTROL_RAW][numpy dynamics path]
+static void* (*const select_step_kernel_of[2][2][2])(int, bool, bool, bool, bool, bool) = {
+    {{qs::select_step_kernel, qs_npy::select_step_kernel}, {qs_pc::select_step_kernel, qs_pc_npy::select_step_kernel}},
+    {{qs_ds::select_step_kernel, qs_ds_npy::select_step_kernel}, {qs_ds_pc::select_step_kernel, qs_ds_pc_npy::select_step_kernel}}};
 
 struct StepShape {
     KernelFn fn;
@@ -481,7 +532,7 @@ static int courier_workers(QsHandle* h, KernelFn fn, int wpc_even) {
 //    4 workers + courier (160 threads, up to three per SM) instead of 128 CTAs of 8 + 1.
 //  * otherwise: 64-thread single-warp CTAs over as many waves as it takes.
 // DYN, NZ and the control modes run in the single-warp shape with the grid-wide wait only; the kernel comes from the
-// select_step_kernel of the handle's control mode and dynamics path.  Host logic only; the CUDA calls are the occupancy
+// select_step_kernel of the handle's dynamics sampler, control mode and dynamics path.  Host logic only; the CUDA calls are the occupancy
 // queries of a handle's first hand-over and courier decisions, whose errors it returns.
 static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const int NP = h->NP, sms = h->sms;
@@ -500,7 +551,8 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const bool scn = p.use_obst ? ticked_obst
                                 : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
                                    p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
-    const auto select = select_step_kernel_of[ctl][h->numpy_dyn ? 1 : 0];     // qs_set_control, qs_set_numpy_dynamics
+    // qs_set_dynamics_sampler, qs_set_control, qs_set_numpy_dynamics
+    const auto select = select_step_kernel_of[h->dyn_spec != nullptr ? 1 : 0][ctl][h->numpy_dyn ? 1 : 0];
     auto kernel = [&](bool ho, bool k_dyn, bool k_nz) { return (KernelFn)select(NP, s.split, scn, ho, k_dyn, k_nz); };
     // A balanced grid that will carry the courier warp (the hand-over is, or will be, chosen below): its worker warps per CTA
     // come from the kernel's occupancy (courier_workers), and the env -> block mapping follows them.
@@ -549,6 +601,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
 }
 
 static int launch_pregen(QsHandle* h, cudaStream_t s);
+static int launch_dyn_pregen(QsHandle* h, cudaStream_t s, const uint8_t* env_mask, bool ahead);
 
 static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool obs_in_device_memory = true) {
     if (h->err_host && *(volatile int*)h->err_host != 0)
@@ -594,10 +647,38 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     h->launches += 1;
     h->started = true;
     note_async(h, s, true);
+    if (h->dyn_every > 0) return launch_dyn_pregen(h, s, nullptr, false);    // the rows this grid's resets did not find
+    return QS_OK;
+}
+
+// The dynamics sampler's rows ahead of the resets (qs_dyn_pregen_kernel); env_mask != null: before an explicit reset of
+// those envs.
+static int launch_dyn_pregen(QsHandle* h, cudaStream_t s, const uint8_t* env_mask, bool ahead) {
+    StepParams p;
+    fill_params(h, p);
+    p.env_mask = env_mask;
+    const int kBlock = 128;
+    const int envs_per_block = kBlock / h->NP;
+    const int grid = (h->cfg.num_envs + envs_per_block - 1) / envs_per_block;
+    int rc = dispatch_np(h->NP, [&](auto np) {
+        if (ahead) qs_dyn_pregen_kernel<decltype(np)::value, true><<<grid, kBlock, 0, s>>>(p);
+        else qs_dyn_pregen_kernel<decltype(np)::value, false><<<grid, kBlock, 0, s>>>(p);
+        return QS_OK;
+    });
+    if (rc != QS_OK) return rc;
+    QS_CUDA(cudaGetLastError());
+    h->launches += 1;
+    note_async(h, s, false);
     return QS_OK;
 }
 
 static int launch_pregen(QsHandle* h, cudaStream_t s) {
+    if (h->dyn_spec != nullptr) {               // the dynamics sampler's rows of the next due episodes
+        const int rc = launch_dyn_pregen(h, s, nullptr, true);
+        if (rc != QS_OK) return rc;
+        h->since_pregen = 0;
+        if (h->cfg.scenario == QS_SCENARIO_HOST_TABLES) return QS_OK;
+    }
     StepParams p;
     fill_params(h, p);
     const int kBlock = 128;
@@ -952,6 +1033,7 @@ extern "C" int qs_set_obstacle_randomization(QsHandle* h, const float* densities
 extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const float* rows_dev, int at_next_reset, void* stream) {
     if (!h || !rows_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
     if (((uintptr_t)rows_dev & 15u) != 0) return fail(QS_ERR_INVALID_ARG, "rows must be 16-byte aligned");
+    if (h->dyn_spec != nullptr) return fail(QS_ERR_INVALID_ARG, "the rows of this handle belong to its dynamics sampler (qs_set_dynamics_sampler)");
     DevState& st = h->st;
     const long long A = h->A, E = h->cfg.num_envs;
     if (st.dyn == nullptr) {
@@ -976,6 +1058,98 @@ extern "C" int qs_set_dynamics(QsHandle* h, const uint8_t* env_mask_dev, const f
     const long long n = A * (QS_DYN_ROW / 4);
     return launch_table(h, stream, n > E ? n : E, k_set_dynamics, st, h->cfg.num_envs, h->cfg.num_agents, env_mask_dev,
                         (const float4*)rows_dev, at_next_reset ? 1 : 0);
+}
+
+// The spec of qs_set_dynamics_sampler is one the sampler can run: known kinds, a tree with every leaf quad_link and the limits
+// read, the walk order a permutation of its leaves, overrides only of leaves it has, finite values.  Empty string = valid.
+static std::string check_dyn_spec(const QsDynSampler& sp) {
+    const uint8_t* P = sp.params.present;
+    if (sp.base != QS_DYN_BASE_FIXED && sp.base != QS_DYN_BASE_RANDOM_QUAD) return "unknown base set";
+    for (int k = 0; k < QS_DYN_LEAVES; ++k) {
+        const bool optional = k == QS_DL_ARMS_L || k == QS_DL_BODY_M || k == QS_DL_BODY_DENSITY || k == QS_DL_PAYLOAD_M ||
+                              k == QS_DL_PAYLOAD_DENSITY || k == QS_DL_ARMS_M || k == QS_DL_ARMS_DENSITY || k == QS_DL_MOTORS_M ||
+                              k == QS_DL_MOTORS_DENSITY || k == QS_DL_PROPS_M || k == QS_DL_PROPS_DENSITY;
+        if (P[k] > 1 || sp.change.present[k] > 1 || sp.samp[0].present[k] > 1 || sp.samp[1].present[k] > 1)
+            return "presence flags must be 0 or 1";
+        if (!optional && !P[k]) return "the parameter tree lacks a leaf the model needs (leaf " + std::to_string(k) + ")";
+        const bool rq_leaf = !(k == QS_DL_ARMS_L || k == QS_DL_BODY_M || k == QS_DL_PAYLOAD_M || k == QS_DL_ARMS_M ||
+                               k == QS_DL_MOTORS_M || k == QS_DL_PROPS_M);
+        if (sp.base == QS_DYN_BASE_RANDOM_QUAD && P[k] != (rq_leaf ? 1 : 0)) return "the tree of RandomQuad has other leaves";
+        if (sp.base == QS_DYN_BASE_FIXED && P[k] && !std::isfinite(sp.params.value[k])) return "non-finite parameter";
+        if (sp.change.present[k] && (!P[k] || !std::isfinite(sp.change.value[k]))) return "dynamics_change: unknown leaf or non-finite value";
+    }
+    for (const int part : {QS_DL_BODY_M, QS_DL_PAYLOAD_M, QS_DL_ARMS_M, QS_DL_MOTORS_M, QS_DL_PROPS_M})
+        if (!P[part] && !P[part + 1]) return "a part has neither `m` nor `density`";
+    int n_present = 0;
+    for (int k = 0; k < QS_DYN_LEAVES; ++k) n_present += P[k];
+    if (sp.n_order != n_present) return "the walk order must list every leaf of the tree once";
+    uint8_t seen[QS_DYN_LEAVES] = {};
+    for (int o = 0; o < sp.n_order; ++o) {
+        const int k = sp.order[o];
+        if (k < 0 || k >= QS_DYN_LEAVES || !P[k] || seen[k]) return "the walk order must list every leaf of the tree once";
+        seen[k] = 1;
+    }
+    for (int s = 0; s < 2; ++s) {
+        const int kind = sp.sampler[s];
+        if (kind < QS_DYN_SAMPLER_NONE || kind > QS_DYN_SAMPLER_CONST) return "unknown sampler kind";
+        for (int k = 0; k < QS_DYN_LEAVES; ++k) {
+            const bool pr = sp.samp[s].present[k] != 0;
+            if ((kind == QS_DYN_SAMPLER_RELATIVE_NORMAL || kind == QS_DYN_SAMPLER_RELATIVE_UNIFORM) && P[k] != pr)
+                return "a relative sampler needs the noise ratio of exactly the tree's leaves";
+            if (kind == QS_DYN_SAMPLER_CONST && pr && !P[k]) return "ConstValueSampler: unknown leaf";
+            if (kind != QS_DYN_SAMPLER_NONE && pr && !std::isfinite(sp.samp[s].value[k])) return "non-finite sampler value";
+        }
+    }
+    return "";
+}
+
+extern "C" int qs_set_dynamics_sampler(QsHandle* h, const QsDynSampler* spec_host, int randomize_every) {
+    if (!h || !spec_host) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->started) return fail(QS_ERR_INVALID_ARG, "the dynamics sampler can only be set before the first reset or step");
+    if (h->dyn_spec != nullptr) return fail(QS_ERR_INVALID_ARG, "the dynamics sampler is already set");
+    if (h->st.dyn != nullptr) return fail(QS_ERR_INVALID_ARG, "this handle already has rows from qs_set_dynamics");
+    if (randomize_every < 0) return fail(QS_ERR_INVALID_ARG, "randomize_every must be >= 0 (0 = construction sample only)");
+    const std::string why = check_dyn_spec(*spec_host);
+    if (!why.empty()) return fail(QS_ERR_INVALID_ARG, "dynamics sampler: " + why);
+    QS_CUDA(cudaSetDevice(h->device));
+    const long long A = h->A, E = h->cfg.num_envs;
+    float4 *d0 = nullptr, *d1 = nullptr;
+    int* pend = nullptr;
+    DynSampler* spec = nullptr;
+    QS_CUDA(dev_alloc(h, &d0, sizeof(float) * QS_DYN_ROW * A));
+    QS_CUDA(dev_alloc(h, &d1, sizeof(float) * QS_DYN_ROW * A));
+    QS_CUDA(dev_alloc(h, &pend, sizeof(int) * E));
+    QS_CUDA(dev_alloc(h, &spec, sizeof(DynSampler)));
+    DynSampler ds;
+    memset(&ds, 0, sizeof(ds));
+    ds.spec = *spec_host;
+    ds.every = randomize_every;
+    QS_CUDA(cudaMemcpy(spec, &ds, sizeof(DynSampler), cudaMemcpyHostToDevice));
+    StepParams p;
+    fill_params(h, p);
+    p.st.dyn = d0;
+    p.dyn = spec;
+    k_dyn_construct<<<(int)((A + 127) / 128), 128>>>(p);
+    QS_CUDA(cudaGetLastError());
+    QS_CUDA(cudaStreamSynchronize(0));
+    h->launches += 1;
+    h->st.dyn = d0; h->st.next_dyn = d1; h->st.dyn_pending = pend;      // published once complete
+    h->dyn_spec = spec;
+    h->dyn_every = randomize_every;
+    if (h->pregen_every == 0 && randomize_every > 0) {       // host-table handles: the generator runs for the sampler alone
+        const char* pg = getenv("QS_PREGEN");
+        h->pregen_every = pg ? atoi(pg) : (h->ep_len / 4 < 16 ? 16 : (h->ep_len / 4 > 256 ? 256 : h->ep_len / 4));
+    }
+    return QS_OK;
+}
+
+extern "C" int qs_get_dynamics(QsHandle* h, float* rows_dev, void* stream) {
+    if (!h || !rows_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (h->st.dyn == nullptr) return fail(QS_ERR_INVALID_ARG, "this handle has no per-drone rows (qs_set_dynamics / qs_set_dynamics_sampler)");
+    QS_CUDA(cudaSetDevice(h->device));
+    QS_CUDA(cudaMemcpyAsync(rows_dev, h->st.dyn, sizeof(float) * QS_DYN_ROW * h->A, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    note_async(h, (cudaStream_t)stream, false);
+    return QS_OK;
 }
 
 extern "C" int qs_set_init_random_state(QsHandle* h, int enable, float vel_max, float omega_max) {
@@ -1096,7 +1270,9 @@ extern "C" int qs_reset(QsHandle* h, const uint8_t* env_mask_dev, float* obs_dev
     fill_params(h, p);
     p.obs = obs_dev;
     p.env_mask = env_mask_dev;
-    int rc = launch_reset(h, p, (cudaStream_t)stream);
+    int rc = QS_OK;
+    if (h->dyn_spec != nullptr) rc = launch_dyn_pregen(h, (cudaStream_t)stream, env_mask_dev, true);      // the rows this reset latches
+    if (rc == QS_OK) rc = launch_reset(h, p, (cudaStream_t)stream);
     if (rc == QS_OK && h->pregen_every > 0) rc = launch_pregen(h, (cudaStream_t)stream);
     return rc;
 }
@@ -1124,7 +1300,19 @@ extern "C" int qs_rollout(QsHandle* h, int num_steps, const float* actions_dev, 
     p.actions = (const float4*)actions_dev;
     p.obs = obs_dev; p.rewards = rewards_dev; p.dones = dones_dev; p.rew_terms = nullptr;
     p.T = num_steps; p.last_obs_only = last_obs_only ? 1 : 0;
-    return launch_step(h, p, (cudaStream_t)stream);
+    if (h->dyn_spec == nullptr) return launch_step(h, p, (cudaStream_t)stream);
+    // dynamics sampler: one grid per control step (a row a reset did not find prepared is sampled behind the grid)
+    const long long A = h->A;
+    p.T = 1;
+    for (int t = 0; t < num_steps; ++t) {
+        StepParams q = p;
+        q.actions = (const float4*)actions_dev + t * A;
+        q.obs = obs_dev + (last_obs_only ? 0 : t * A * h->D);
+        q.rewards = rewards_dev + t * A; q.dones = dones_dev + t * A;
+        const int rc = launch_step(h, q, (cudaStream_t)stream);
+        if (rc != QS_OK) return rc;
+    }
+    return QS_OK;
 }
 
 // true when the host pointer is page-locked (cudaHostAlloc / cudaHostRegister): DMA can use it directly.  `dev` receives the

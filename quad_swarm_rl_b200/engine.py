@@ -59,7 +59,8 @@ class QuadSwarmEngine:
                  collision_hitbox_radius=2.0, collision_falloff_radius=4.0, sense_noise='default',
                  approch_goal_metric=0.5, rew_coeff=None, seed=0, device=0, env_id_offset=0,
                  device_scenario=None, quad_arm=0.0, init_random_state=False, init_vel_max=1.0, init_omega_max=2 * math.pi,
-                 use_numba=True, raw_control=True, raw_control_zero_middle=True):
+                 use_numba=True, raw_control=True, raw_control_zero_middle=True, dynamics_sampler=None,
+                 dynamics_randomize_every=None):
         if not torch.cuda.is_available():
             raise RuntimeError("QuadSwarmEngine needs a CUDA device (the env step has no CPU path)")
         self.lib = L.load()
@@ -118,6 +119,11 @@ class QuadSwarmEngine:
             L.check(self.lib.qs_set_control(h, L.QS_CONTROL_POSITION))
         elif not self.raw_control_zero_middle:
             L.check(self.lib.qs_set_control(h, L.QS_CONTROL_RAW_UNIT))
+        # dynamics randomisation on the device (quad_models.dynamics_sampler_spec): every drone's row is sampled at
+        # construction and at the resets `dynamics_randomize_every` names (quadrotor_single.py:186-211,359-390)
+        if dynamics_sampler is not None:
+            spec = L.dyn_sampler_struct(dynamics_sampler)
+            L.check(self.lib.qs_set_dynamics_sampler(h, C.byref(spec), int(dynamics_randomize_every or 0)))
         self.D = self.lib.qs_obs_dim(h)
         self.M = self.lib.qs_num_obstacles(h)
         self.ep_len = self.lib.qs_ep_len(h)
@@ -285,6 +291,12 @@ class QuadSwarmEngine:
         ags = torch.empty((self.E, self.N, L.QS_NUM_AGENT_STATS), dtype=torch.float32, device=dev)
         L.check(self.lib.qs_read_episode_stats(self.h, _ptr(es), _ptr(ags), self._stream()))
         return es, ags
+
+    def get_dynamics(self):
+        """The live per-drone rows [E,N,QS_DYN_ROW] (qs_get_dynamics)."""
+        out = torch.empty((self.E, self.N, L.QS_DYN_ROW), dtype=torch.float32, device=self.device)
+        L.check(self.lib.qs_get_dynamics(self.h, _ptr(out), self._stream()))
+        return out
 
     def set_dynamics(self, rows, env_mask=None, at_next_reset=False):
         """Per-drone physical constants (include/quadswarm.h, qs_set_dynamics): rows [E,N,QS_DYN_ROW] float32, the layout

@@ -83,7 +83,7 @@ class _EnvBase:
                  use_downwash, use_numba, quads_mode, room_dims, use_replay_buffer, quads_view_mode, quads_render,
                  dynamics_params, raw_control, raw_control_zero_middle, dynamics_randomize_every, dynamics_change,
                  dyn_sampler_1, sense_noise, init_random_state, render_mode='human', device=0, seed=None,
-                 env_id_offset=0, device_scenario=None):
+                 env_id_offset=0, device_scenario=None, device_dynamics=False):
         # the env factory's fixed choices (swarm_rl/env_wrappers/quad_utils.py:22-31) are the only supported ones
         from .quad_models import SAMPLERS
         if isinstance(dynamics_params, str) and dynamics_params not in SAMPLERS:
@@ -141,14 +141,32 @@ class _EnvBase:
         factory_change = dict(noise=dict(thrust_noise_ratio=0.05), damp=dict(vel=0, omega_quadratic=0))      # quad_utils.py:31
         self.dynamics_randomize_every = dynamics_randomize_every
         self._dyn_sources = None
+        dyn_spec, t2w = None, None
         quad_arm = 0.0
         if dynamics_params != 'Crazyflie' or dyn_sampler_1 is not None or dynamics_randomize_every is not None or \
                 (dynamics_change is not None and dynamics_change != factory_change):
-            from .quad_models import DynamicsSource, DYN_FIELDS
-            self._dyn_sources = [DynamicsSource(dynamics_params, dynamics_change, dyn_sampler_1, rs=self._host_rng)
-                                 for _ in range(self.num_envs * num_agents)]
-            self._dyn_rows = np.stack([src.sample_row() for src in self._dyn_sources]).reshape(self.num_envs, num_agents, -1)
-            quad_arm = float(self._dyn_rows[0, 0, DYN_FIELDS.index('arm')])          # quadrotor_multi.py:81: envs[0].dynamics.arm
+            from .quad_models import DynamicsSource, DYN_FIELDS, GRAV, dynamics_sampler_spec
+            if device_dynamics:
+                # the sampler runs on the device (qs_set_dynamics_sampler); quad_arm and envs[0]'s thrust-to-weight come from
+                # the construction row of env 0, drone 0.  That row depends on (seed, env id, episode 0, drone 0) only, so a
+                # one-env handle with the same seed and env id computes it before the real handle, whose QsConfig.quad_arm
+                # needs it.  The thrust-to-weight is recovered from the float32 row (sum of thrust_max / (g mass)): it
+                # differs from the parameter itself by about 1e-7 relative (it only sets the position controller's action
+                # bounds).
+                dyn_spec = dynamics_sampler_spec(dynamics_params, dynamics_change, dyn_sampler_1)
+                probe = QuadSwarmEngine(num_envs=1, num_agents=num_agents, seed=seed, device=device, env_id_offset=env_id_offset,
+                                        dynamics_sampler=dyn_spec)
+                row0 = probe.get_dynamics()[0, 0].double().cpu().numpy()
+                probe.close()
+                F = DYN_FIELDS.index
+                t2w = float(row0[F('thrust_max0'):F('thrust_max3') + 1].sum() / (GRAV * row0[F('mass')]))
+            else:
+                self._dyn_sources = [DynamicsSource(dynamics_params, dynamics_change, dyn_sampler_1, rs=self._host_rng)
+                                     for _ in range(self.num_envs * num_agents)]
+                self._dyn_rows = np.stack([src.sample_row() for src in self._dyn_sources]).reshape(self.num_envs, num_agents, -1)
+                row0 = self._dyn_rows[0, 0]
+                t2w = self._dyn_sources[0].params['motor']['thrust_to_weight']
+            quad_arm = float(row0[DYN_FIELDS.index('arm')])          # quadrotor_multi.py:81: envs[0].dynamics.arm
             self.quad_arm = quad_arm
             self.collision_threshold = collision_hitbox_radius * quad_arm
             self.collision_falloff_threshold = collision_falloff_radius * quad_arm
@@ -161,7 +179,8 @@ class _EnvBase:
             collision_falloff_radius=collision_falloff_radius, sense_noise=sense_noise, rew_coeff=rew_coeff,
             seed=seed, device=device, env_id_offset=env_id_offset, device_scenario=device_scenario, quad_arm=quad_arm,
             init_random_state=init_random_state, use_numba=bool(use_numba), raw_control=self.raw_control,
-            raw_control_zero_middle=self.raw_control_zero_middle,
+            raw_control_zero_middle=self.raw_control_zero_middle, dynamics_sampler=dyn_spec,
+            dynamics_randomize_every=dynamics_randomize_every,
             # scenario.approch_goal_metric (o_base.py:16: 1.0 for the goal-sharing obstacle scenarios, else 0.5); with the
             # host-side `mix` over obstacle scenarios the value of o_random is used for every episode
             approch_goal_metric=1.0 if quads_mode in ('o_static_same_goal', 'o_dynamic_same_goal', 'o_swap_goals',
@@ -180,8 +199,9 @@ class _EnvBase:
         self.num_obstacles = self.engine.M
         self.observation_space = make_observation_space(obs_repr, k_eff, self.use_obstacles, room_dims)
         # envs[0]'s action space (quadrotor_multi.py): the position controller's bounds depend on its model's thrust_to_weight
-        from .quad_models import crazyflie_params
-        t2w = (crazyflie_params() if self._dyn_sources is None else self._dyn_sources[0].params)['motor']['thrust_to_weight']
+        if t2w is None:
+            from .quad_models import crazyflie_params
+            t2w = crazyflie_params()['motor']['thrust_to_weight']
         self.action_space = make_action_space(self.raw_control, self.raw_control_zero_middle, t2w)
         assert self.observation_space.shape[0] == self.engine.D == obs_self_size + 6 * k_eff + (9 if self.use_obstacles else 0)
         # host-side episode generators: the scenario of the current episode and of the next one, per env
@@ -483,7 +503,11 @@ class QuadrotorEnvMultiBatched(_EnvBase):
                  room_dims=(10., 10., 10.), sense_noise='default', device=0, seed=None, env_id_offset=0,
                  device_scenarios=True, dynamics_params='Crazyflie', dynamics_randomize_every=None, dynamics_change=None,
                  dyn_sampler_1=None, init_random_state=False, use_numba=True, raw_control=True,
-                 raw_control_zero_middle=True):
+                 raw_control_zero_middle=True, device_dynamics=False):
+        """device_dynamics: who produces the per-drone physical constants, like device_scenarios for the episodes.  False:
+        one host quad_models.DynamicsSource per drone, re-uploaded every ep_len + 1 steps when dynamics_randomize_every is
+        set.  True: the device samples every drone's row at construction and at each env's own resets
+        (qs_set_dynamics_sampler); nothing is sampled or uploaded on the host."""
         # device-side generators (no host work per episode or per tick): o_random with obstacles, the goal-formation
         # family and mix without; every other mode uses host tables
         dev_scn = None
@@ -495,7 +519,8 @@ class QuadrotorEnvMultiBatched(_EnvBase):
                          collision_hitbox_radius, collision_falloff_radius, use_obstacles, obst_density, obst_size,
                          obst_spawn_area, use_downwash, use_numba, quads_mode, room_dims, False, ['topdown'], False,
                          dynamics_params, raw_control, raw_control_zero_middle, dynamics_randomize_every, dynamics_change, dyn_sampler_1, sense_noise,
-                         init_random_state, device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn)
+                         init_random_state, device=device, seed=seed, env_id_offset=env_id_offset, device_scenario=dev_scn,
+                         device_dynamics=device_dynamics)
         self.num_agents = num_envs * num_agents
         self._truncated = torch.zeros(self.num_agents, dtype=torch.bool, device=self.engine.device)
 

@@ -10,6 +10,9 @@ Here the same pipeline ends in one float32 row per drone (`derive_constants` -> 
 `qs_set_dynamics` uploads; the step kernel reads the row instead of compile-time Crazyflie constants.  The samplers draw
 from a `numpy.random.RandomState` in the reference's call order, so that, seeded alike, they reproduce the reference's
 parameter sets (tests/golden/dyn_models.json pins them).
+
+`dynamics_sampler_spec` turns the same arguments into the flat leaf vector of qs_set_dynamics_sampler, with which the
+device runs this pipeline itself, per drone and per episode, from keyed draws (csrc/qs_dyn_sampler.cuh).
 """
 import copy
 import math
@@ -338,3 +341,122 @@ class DynamicsSource:
     def sample_row(self):
         self.params = self.sample()          # the parameter set of the row (its thrust_to_weight bounds the controller's actions)
         return constants_row(self.params)
+
+
+# ---- the flat spec of the device-side sampler (QsDynSampler, include/quadswarm.h; qs_set_dynamics_sampler) ------------------
+# Leaf id -> (path in the parameter tree, element of an array leaf or None); the order is QS_DL_* of the header.
+DYN_LEAVES = tuple(
+    [(('geom', part, k), None) for part in ('body', 'payload', 'arms') for k in ('l', 'w', 'h', 'm', 'density')] +
+    [(('geom', part, k), None) for part in ('motors', 'propellers') for k in ('h', 'r', 'm', 'density')] +
+    [(('geom', 'motor_pos', 'xyz'), e) for e in range(3)] +
+    [(('geom', 'arms_pos', 'angle'), None), (('geom', 'arms_pos', 'z'), None)] +
+    [(('geom', 'payload_pos', 'xy'), e) for e in range(2)] + [(('geom', 'payload_pos', 'z_sign'), None)] +
+    [(('damp', 'vel'), None), (('damp', 'omega_quadratic'), None), (('noise', 'thrust_noise_ratio'), None),
+     (('motor', 'thrust_to_weight'), None)] + [(('motor', 'assymetry'), e) for e in range(4)] +
+    [(('motor', k), None) for k in ('torque_to_thrust', 'linearity', 'C_drag', 'C_roll', 'damp_time_up', 'damp_time_down')])
+DYN_NUM_LEAVES = len(DYN_LEAVES)                 # QS_DYN_LEAVES
+_LEAF_IDS = {}
+for _k, (_path, _e) in enumerate(DYN_LEAVES):
+    _LEAF_IDS.setdefault(_path, []).append(_k)
+DYN_BASE_FIXED, DYN_BASE_RANDOM_QUAD = 0, 1
+DYN_SAMPLER_NONE, DYN_SAMPLER_RELATIVE_NORMAL, DYN_SAMPLER_RELATIVE_UNIFORM, DYN_SAMPLER_CONST = 0, 1, 2, 3
+
+
+def flatten_tree(tree, broadcast=False):
+    """Parameter tree (or a partial one: dynamics_change, a ConstValueSampler's change, noise ratios) -> (present [L] uint8,
+    value [L] float64, order: the leaf ids in the order the tree is walked, i.e. the order RelativeSampler draws in).
+    broadcast: a number stands for every element of an array leaf (RelativeSampler's noise ratios).  Raises ValueError for a
+    leaf the device cannot represent."""
+    present = np.zeros(DYN_NUM_LEAVES, np.uint8)
+    value = np.zeros(DYN_NUM_LEAVES, np.float64)
+    order = []
+
+    def visit(node, path):
+        if not isinstance(node, dict):
+            raise ValueError("dynamics parameters must be a dict")
+        for key, item in node.items():
+            p = path + (key,)
+            if isinstance(item, dict):
+                visit(item, p)
+                continue
+            ids = _LEAF_IDS.get(p)
+            if ids is None:
+                raise ValueError(f"dynamics parameters: the device sampler has no leaf {'.'.join(p)}")
+            vals = np.asarray(item, dtype=object).ravel()
+            if broadcast and np.ndim(item) == 0:
+                vals = np.repeat(vals, len(ids))
+            elif len(vals) != len(ids) or (DYN_LEAVES[ids[0]][1] is None) != (np.ndim(item) == 0):
+                raise ValueError(f"dynamics parameters: {'.'.join(p)} must be {'a number' if len(ids) == 1 else f'{len(ids)} numbers'}")
+            for k, v in zip(ids, vals):
+                if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not np.isfinite(v):
+                    raise ValueError(f"dynamics parameters: {'.'.join(p)} = {item!r} is not a finite number")
+                present[k], value[k] = 1, float(v)
+                order.append(k)
+
+    visit(tree, ())
+    return present, value, order
+
+
+def unflatten_tree(present, value, order):
+    """Inverse of flatten_tree: the tree with the leaves of `order`, in that order (array leaves as lists)."""
+    tree = {}
+    for k in order:
+        assert present[k]
+        path, e = DYN_LEAVES[k]
+        node = tree
+        for key in path[:-1]:
+            node = node.setdefault(key, {})
+        if e is None:
+            node[path[-1]] = float(value[k])
+        else:
+            node.setdefault(path[-1], []).append(float(value[k]))
+    return tree
+
+
+def dynamics_sampler_spec(dynamics_params='Crazyflie', dynamics_change=None, dyn_sampler_1=None, dyn_sampler_2=None):
+    """The QsDynSampler of (dynamics_params, dynamics_change, dyn_sampler_1, dyn_sampler_2), as a dict of numpy arrays
+    (_lib.dyn_sampler_struct packs it).  The tree is the one DynamicsSource builds, so its walk order is the host pipeline's
+    draw order.  Raises ValueError for anything the device sampler cannot run: base sets outside SAMPLERS, samplers other than
+    RelativeSampler / ConstValueSampler, leaves outside DYN_LEAVES, non-finite values."""
+    if isinstance(dynamics_params, str):
+        if dynamics_params not in ('Crazyflie', 'DefaultQuad', 'MediumQuad', 'RandomQuad'):
+            raise ValueError(f"unknown dynamics_params {dynamics_params!r}")
+    elif not isinstance(dynamics_params, dict):
+        raise ValueError("dynamics_params must be a parameter-set name or a dict")
+    for s in (dyn_sampler_1, dyn_sampler_2):
+        if s is not None and (not isinstance(s, dict) or s.get('class') not in ('RelativeSampler', 'ConstValueSampler')):
+            raise ValueError(f"the device sampler supports RelativeSampler and ConstValueSampler, not {s!r}")
+        if s is not None and s['class'] == 'RelativeSampler' and s.get('sampler', 'normal') not in ('normal', 'uniform'):
+            raise ValueError(f"RelativeSampler(sampler={s['sampler']!r}): 'normal' or 'uniform'")
+    try:
+        src = DynamicsSource(dynamics_params, dynamics_change, dyn_sampler_1, dyn_sampler_2, rs=np.random.RandomState(0))
+        tree = src._base()                   # the tree the samplers walk (for RandomQuad: its structure; values unused)
+    except (KeyError, TypeError) as e:
+        raise ValueError(f"dynamics parameters the host pipeline cannot build: {e!r}") from None
+    base = src.fixed if src.fixed is not None else src.base.sample(rs=np.random.RandomState(0))      # without dynamics_change
+    present, value, order = flatten_tree(base)
+    if flatten_tree(tree)[2] != order:
+        raise ValueError("dynamics_change must not reorder the parameter tree")
+    random_quad = dynamics_params == 'RandomQuad'
+    spec = dict(base=DYN_BASE_RANDOM_QUAD if random_quad else DYN_BASE_FIXED, order=np.array(order, np.int32),
+                params=(present, np.zeros_like(value) if random_quad else value),
+                change=flatten_tree(dynamics_change)[:2] if dynamics_change is not None else
+                (np.zeros(DYN_NUM_LEAVES, np.uint8), np.zeros(DYN_NUM_LEAVES)), sampler=[], samp=[])
+    if not np.all(spec['change'][0] <= present):
+        raise ValueError("dynamics_change names a leaf the parameter tree does not have")
+    for s, obj in ((dyn_sampler_1, src.s1), (dyn_sampler_2, src.s2)):
+        if s is None:
+            spec['sampler'].append(DYN_SAMPLER_NONE)
+            spec['samp'].append((np.zeros(DYN_NUM_LEAVES, np.uint8), np.zeros(DYN_NUM_LEAVES)))
+        elif isinstance(obj, RelativeSampler):
+            spec['sampler'].append(DYN_SAMPLER_RELATIVE_NORMAL if obj.sampler == 'normal' else DYN_SAMPLER_RELATIVE_UNIFORM)
+            pr, ratio, _ = flatten_tree(obj.noise_params, broadcast=True)
+            spec['samp'].append((pr, ratio))
+        else:
+            pr, val, _ = flatten_tree(obj.params_change)
+            if not np.all(pr <= present):
+                raise ValueError("ConstValueSampler names a leaf the parameter tree does not have")
+            spec['sampler'].append(DYN_SAMPLER_CONST)
+            spec['samp'].append((pr, val))
+    return spec
+
