@@ -295,10 +295,10 @@ typedef struct QsDynSampler {
  * construction sample.  randomize_every = 0 is the reference's None (the construction sample only).  Later calls, a handle
  * that already has rows from qs_set_dynamics, malformed specs (unknown kinds, leaves outside the tree, missing leaves the
  * model needs) and non-finite values fail with QS_ERR_INVALID_ARG.  qs_set_dynamics fails on such a handle: the sampler owns
- * the rows.  The sampling runs ahead of the resets where it can (beside the next-episode generator, before an explicit
- * reset) and otherwise right behind the step grid whose reset needs the row, with the same results.  A sampler handle
- * steps with DYN kernels of its own (single-warp shape, grid-wide wait), one control step per grid: its qs_rollout launches
- * num_steps grids. */
+ * the rows.  The sampling runs ahead of the resets where it can (beside the next-episode generator); the new rows are
+ * latched right behind the step grid or the qs_reset that started their episode, and sampled there if none were prepared,
+ * with the same results.  A sampler handle steps with the DYN kernels of qs_set_dynamics (single-warp shape, grid-wide
+ * wait), one control step per grid: its qs_rollout launches num_steps grids. */
 int qs_set_dynamics_sampler(QsHandle* h, const QsDynSampler* spec_host, int randomize_every);
 /* The live rows of every drone, rows_dev [E,N,QS_DYN_ROW] floats (device -> device copy on `stream`).  Fails on a handle
  * without per-drone rows (neither qs_set_dynamics nor qs_set_dynamics_sampler was called). */

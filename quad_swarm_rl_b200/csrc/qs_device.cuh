@@ -49,11 +49,6 @@ constexpr float FLOOR_THRESHOLD_NP = 0.05f;       // floor threshold and snap he
 #ifndef QS_CONTROL_MODES
 #define QS_CONTROL_MODES 0
 #endif
-// QS_DYN_SAMPLER = 1 (set by the qs_step_ds*.cu units only): the DYN step kernels of handles with the device-side dynamics
-// sampler (qs_set_dynamics_sampler; the sampler's reset path in qs_step_kernel).
-#ifndef QS_DYN_SAMPLER
-#define QS_DYN_SAMPLER 0
-#endif
 constexpr float SIM_DT = 0.005f;                  // quadrotor_single.py:157
 constexpr float CONTROL_DT = 0.01f;               // quadrotor_multi.py:83
 constexpr int SIM_STEPS = 2;                      // quadrotor_single.py:102
@@ -104,8 +99,10 @@ struct DevState {
     int4* next_scn_i;       // [E]     scenario state of the pre-generated next episode
     float4* next_scn_f;     // [E][3]
     float4* dyn;            // [A][QS_DYN_ROW / 4] per-drone physical constants (qs_set_dynamics), or null: Crazyflie constants
-    float4* next_dyn;       // [A][QS_DYN_ROW / 4] constants latched by the env's next (auto-)reset when dyn_pending[env] != 0
-    int* dyn_pending;       // [E]
+    float4* next_dyn;       // [A][QS_DYN_ROW / 4] constants latched by the env's next (auto-)reset when dyn_pending[env] != 0;
+                            //     dynamics sampler: the rows qs_dyn_pregen_kernel prepared for episode dyn_pending[E + env]
+    int* dyn_pending;       // [E]; dynamics sampler: [2][E], row 0 always 0 (the step and reset kernels latch nothing),
+                            //     row 1 the episode whose rows next_dyn holds, 0 = none
     int* err_flag;          // mapped page-locked host word: set to 1 by a step kernel whose hand-over wait timed out (sticky)
     int4* scn_i;            // [E]     device-side scenario state: scenario, period, next event tick, formation | growing << 8
     float4* scn_f;          // [E][3]  formation size / layer distance / largest size / speed; centre 1; centre 2
@@ -168,8 +165,8 @@ struct StepParams {
     int init_random;                    // qs_set_init_random_state: every spawn gets a random vel / omega / R (random_init_state)
     float init_vel_max, init_omega_max;
     int control;                        // qs_set_control: QS_CONTROL_*; read only by the kernels of qs_step_pc.cu
-    const DynSampler* dyn;              // qs_set_dynamics_sampler (qs_dyn_sampler.cuh), or null; read only by the DYN
-                                        // instantiations and the sampler's kernels.  It takes the last 8 bytes of the
+    const DynSampler* dyn;              // qs_set_dynamics_sampler (qs_dyn_sampler.cuh), or null; read only by the
+                                        // sampler's kernels (quadswarm.cu).  It takes the last 8 bytes of the
                                         // struct's padding: every other kernel keeps its parameter layout.
 };
 

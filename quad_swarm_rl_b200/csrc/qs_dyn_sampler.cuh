@@ -143,8 +143,7 @@ __device__ __forceinline__ void quad_link_part(const double* L, const uint8_t* P
 }
 
 // quad_link + derive_constants (quad_models.py:62-143) -> the row (DYN_FIELDS), still in float64.  The 14 links go through
-// a table in local memory and rolled loops: a rare path, kept to few registers so that the step kernels calling
-// sample_dyn_row keep theirs.
+// a table in local memory and rolled loops: a rare path, kept to few registers.
 __device__ __forceinline__ void derive_row(const double* L, const uint8_t* P, double* row) {
     double angle = L[QS_DL_ARMS_ANGLE] / 180. * 3.141592653589793;
     if (angle == 0.) angle = 0.01;
@@ -202,8 +201,8 @@ __device__ __forceinline__ void derive_row(const double* L, const uint8_t* P, do
 }
 
 // DynamicsSource.sample() + derive_constants for drone i under `key` (the episode key of the env's episode that starts, or
-// episode 0 for the construction sample); writes the float32 row to `out` (QS_DYN_ROW / 4 float4).  Out of line: the step
-// kernels call it only at a resampling reset whose row was not prepared ahead of time.
+// episode 0 for the construction sample); writes the float32 row to `out` (QS_DYN_ROW / 4 float4).  Called by the sampler's
+// own kernels only (k_dyn_construct, qs_dyn_pregen_kernel), never by a step kernel.
 __device__ __noinline__ void sample_dyn_row(const DynSampler* __restrict__ dyn, RngKey key, int i, float4* out) {
     const QsDynSampler* __restrict__ spec = &dyn->spec;
     double L[QS_DYN_LEAVES], L0[QS_DYN_LEAVES];

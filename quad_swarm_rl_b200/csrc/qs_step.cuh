@@ -1230,43 +1230,21 @@ __global__ void __launch_bounds__(step_max_threads<NP, SPLIT, SCN, HO, DYN, NZ>(
                                p.init_random != 0);
             if (DYN) {
                 // resample_dynamics inside _reset (quadrotor_single.py:387-390): constants uploaded with at_next_reset are
-                // latched now; update_dynamics builds a fresh QuadrotorDynamics, so OU state and SVD counter restart
+                // latched now; update_dynamics builds a fresh QuadrotorDynamics, so OU state and SVD counter restart.  A
+                // handle with the device-side sampler never has a row pending: qs_dyn_pregen_kernel latches its rows.
                 const int pend = do_reset ? QS_LD(st.dyn_pending + env) : 0;
-#if QS_DYN_SAMPLER
-                // device-side sampler (qs_set_dynamics_sampler): the resets its cadence names latch the row
-                // qs_dyn_pregen_kernel prepared for their episode (dyn_pending = its number).  A row it has not prepared is
-                // marked (dyn_pending = -episode) and sampled by qs_dyn_pregen_kernel right behind this grid: a sampler
-                // handle launches one control step per grid (qs_rollout included), so no later step of this grid needs it,
-                // and the step kernel makes no call to the sampler.
-                __syncwarp();               // lane 0 of the env has stored the number of the episode that starts (reset_env)
-                const int g_dyn = do_reset ? QS_LD(st.epi + env).x : 0;
-                const bool latch = do_reset && dyn_due(g_dyn, __ldg(&p.dyn->every));
-                const int pend_after = (latch && pend != g_dyn) ? -g_dyn : 0;
-                if (latch) {
-                    if (valid) {
-                        if (pend == g_dyn) {
-                            for (int q = 0; q < QS_DYN_ROW / 4; ++q)
-                                st.dyn[a * (QS_DYN_ROW / 4) + q] = QS_LD(st.next_dyn + a * (QS_DYN_ROW / 4) + q);
-                            load_phys(st.next_dyn, a, ph);
-                        }
-#else
                 if (pend != 0) {
                     if (valid) {
                         for (int q = 0; q < QS_DYN_ROW / 4; ++q)
                             st.dyn[a * (QS_DYN_ROW / 4) + q] = QS_LD(st.next_dyn + a * (QS_DYN_ROW / 4) + q);
                         load_phys(st.next_dyn, a, ph);
-#endif
 #pragma unroll
                         for (int k = 0; k < 4; ++k) s.ou[k] = 0.f;
                     }
                     ctr.svd_count = 0;
                 }
                 __syncwarp();
-#if QS_DYN_SAMPLER
-                if (pend != pend_after && i == 0) st.dyn_pending[env] = pend_after;
-#else
                 if (pend != 0 && i == 0) st.dyn_pending[env] = 0;
-#endif
             }
 #ifdef QS_TIMELINE
             if (__float_as_int(s.pos[0]) == 0x7fffffff) QS_TL(7);

@@ -1,7 +1,6 @@
 // Which step-kernel instantiation a launch takes (host code).  Every translation unit with step kernels includes this file
 // and so exports select_step_kernel in its own namespace, over its own qs_step_kernel: qs (quadswarm.cu), qs_npy
-// (qs_step_npy.cu), qs_pc and qs_pc_npy (qs_step_pc.cu, qs_step_pc_npy.cu), and the dynamics sampler's qs_ds* units
-// (qs_step_ds*.cu).  plan_step (quadswarm.cu) picks the unit.
+// (qs_step_npy.cu), and qs_pc and qs_pc_npy (qs_step_pc.cu, qs_step_pc_npy.cu).  plan_step (quadswarm.cu) picks the unit.
 #pragma once
 #include "qs_step.cuh"
 
@@ -21,9 +20,6 @@ static KernelFn step_kernel_scn(bool scn) {
 // "Numpy dynamics path"): keep it.
 template <int NP>
 static KernelFn step_kernel(bool split, bool scn, bool ho, bool dyn, bool nz) {
-#if QS_DYN_SAMPLER
-    return nz ? step_kernel_scn<NP, false, false, true, true>(scn) : step_kernel_scn<NP, false, false, true, false>(scn);    // DYN only
-#else
     if (nz) return dyn ? step_kernel_scn<NP, false, false, true, true>(scn) : step_kernel_scn<NP, false, false, false, true>(scn);
     if (dyn) return step_kernel_scn<NP, false, false, true, false>(scn);
     if constexpr (!QS_CONTROL_MODES) {
@@ -31,7 +27,6 @@ static KernelFn step_kernel(bool split, bool scn, bool ho, bool dyn, bool nz) {
         if (ho) return step_kernel_scn<NP, false, true, false, false>(scn);
     }
     return step_kernel_scn<NP, false, false, false, false>(scn);
-#endif
 }
 
 // The step kernel of a launch, as a void* because StepParams is a type of the unit's own namespace.

@@ -404,38 +404,47 @@ __global__ void k_dyn_construct(const __grid_constant__ StepParams p) {
     sample_dyn_row(p.dyn, episode_key(p, env, 0), i, p.st.dyn + t * (QS_DYN_ROW / 4));
 }
 
-// The device-side dynamics sampler around the resets.  AHEAD = false: launched behind every step grid of a sampler handle
-// that resamples; AHEAD = true: beside qs_pregen_kernel (same cadence) and before every explicit reset, on its env mask
-// (p.env_mask).
-//  * dyn_pending = -g: a step grid started episode g, which resamples, without a prepared row: sample it into the live table;
-//  * AHEAD: then, for the episode g = epi.x + 1 the env starts at its next reset: if it resamples (dyn_due) and has no prepared row
-//    yet, sample its rows into next_dyn and tag them with dyn_pending = g, which that reset latches (qs_step_kernel, DYN;
-//    qs_reset_kernel); if it does not, dyn_pending = 0, so that qs_reset_kernel latches nothing (also after the episode
-//    number was set back since a tag was written).
-// Lanes as in qs_pregen_kernel: the drones of an env sit in one warp, which reads the tag before lane 0 rewrites it.
+// The device-side dynamics sampler at the resets: the only kernel that changes the rows of a sampler handle after its
+// construction sample.  The step and reset kernels latch nothing on such a handle (its dyn_pending row 0 stays 0); row 1,
+// `prepared`, holds the episode whose rows next_dyn holds.
+//  * AHEAD (beside qs_pregen_kernel, same cadence): for the episode g = epi.x + 1 the env starts at its next reset: if it
+//    resamples (dyn_due) and next_dyn does not hold its rows yet, sample them into next_dyn and record g.
+//  * behind (right after every step grid of a resampling handle, and after qs_reset's reset kernel on its env mask,
+//    p.env_mask): every env that reset in that launch has tick 0 (a sampler handle runs one control step per grid).  If
+//    the episode g = epi.x it started resamples, its live rows become next_dyn's when those were recorded for g, else
+//    they are sampled for g; and, as update_dynamics builds a fresh QuadrotorDynamics, its OU state and SVD counter
+//    restart.  A record that went stale (qs_set_state moved the episode number) never matches.  Latching here instead of
+//    inside the launch changes no output: in the step kernel nothing after the reset reads the constants, the OU state
+//    or the SVD counter (rewards come before the reset; the observation uses none of them), nor in qs_reset_kernel.
+// Lanes as in qs_pregen_kernel: the drones of an env sit in one warp, which reads the record before lane 0 rewrites it.
 template <int NP, bool AHEAD>
 __global__ void __launch_bounds__(128) qs_dyn_pregen_kernel(const __grid_constant__ StepParams p) {
     const DevState& st = p.st;
     const int i = (threadIdx.x & 31) & (NP - 1);
     const int env = blockIdx.x * (blockDim.x / NP) + threadIdx.x / NP;
     const bool env_ok = env < p.E && (p.env_mask == nullptr || p.env_mask[env] != 0);
-    int g = 0, pend = 0;
-    if (env_ok) {
-        g = st.epi[env].x + 1;
-        pend = st.dyn_pending[env];
-    }
     const long long a = (long long)env * p.N + i;
-    if (pend < 0 && i < p.N) sample_dyn_row(p.dyn, episode_key(p, env, -pend), i, st.dyn + a * (QS_DYN_ROW / 4));
-    if (!AHEAD) {               // behind a step grid: only the rows its resets did not find
+    int* const prepared = st.dyn_pending + p.E;
+    if (AHEAD) {
+        const int g = env_ok ? st.epi[env].x + 1 : 0;
+        const bool sample = env_ok && dyn_due(g, p.dyn->every) && prepared[env] != g;
+        if (sample && i < p.N) sample_dyn_row(p.dyn, episode_key(p, env, g), i, st.next_dyn + a * (QS_DYN_ROW / 4));
         __syncwarp();
-        if (i == 0 && pend < 0) st.dyn_pending[env] = 0;
-        return;
+        if (sample && i == 0) prepared[env] = g;
+    } else {
+        const int g = env_ok ? st.epi[env].x : 0;
+        const bool latch = env_ok && st.env_ctr[env].x == 0 && dyn_due(g, p.dyn->every);
+        if (latch && i < p.N) {
+            float4* const row = st.dyn + a * (QS_DYN_ROW / 4);
+            if (prepared[env] == g) {
+                for (int q = 0; q < QS_DYN_ROW / 4; ++q) row[q] = st.next_dyn[a * (QS_DYN_ROW / 4) + q];
+            } else {
+                sample_dyn_row(p.dyn, episode_key(p, env, g), i, row);
+            }
+            st.slots[SL_OU * st.a_pad + a] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        if (latch && i == 0) st.env_ctr[env].z = 0;
     }
-    const bool due = env_ok && dyn_due(g, p.dyn->every);
-    if (due && pend != g && i < p.N) sample_dyn_row(p.dyn, episode_key(p, env, g), i, st.next_dyn + a * (QS_DYN_ROW / 4));
-    const int pend_after = due ? g : 0;
-    __syncwarp();
-    if (i == 0 && env_ok && pend != pend_after) st.dyn_pending[env] = pend_after;
 }
 
 __global__ void k_read_stats(DevState st, int E, int N, int32_t* env_stats, float* agent_stats) {
@@ -471,16 +480,10 @@ static int dispatch_np(int NP, F&& f) {
 namespace qs_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 namespace qs_pc { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 namespace qs_pc_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
-// the DYN kernels of handles with the device-side dynamics sampler (qs_step_ds*.cu)
-namespace qs_ds { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
-namespace qs_ds_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
-namespace qs_ds_pc { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
-namespace qs_ds_pc_npy { void* select_step_kernel(int NP, bool split, bool scn, bool ho, bool dyn, bool nz); }
 
-// [dynamics sampler][control mode other than QS_CONTROL_RAW][numpy dynamics path]
-static void* (*const select_step_kernel_of[2][2][2])(int, bool, bool, bool, bool, bool) = {
-    {{qs::select_step_kernel, qs_npy::select_step_kernel}, {qs_pc::select_step_kernel, qs_pc_npy::select_step_kernel}},
-    {{qs_ds::select_step_kernel, qs_ds_npy::select_step_kernel}, {qs_ds_pc::select_step_kernel, qs_ds_pc_npy::select_step_kernel}}};
+// [control mode other than QS_CONTROL_RAW][numpy dynamics path]
+static void* (*const select_step_kernel_of[2][2])(int, bool, bool, bool, bool, bool) = {
+    {qs::select_step_kernel, qs_npy::select_step_kernel}, {qs_pc::select_step_kernel, qs_pc_npy::select_step_kernel}};
 
 struct StepShape {
     KernelFn fn;
@@ -532,7 +535,7 @@ static int courier_workers(QsHandle* h, KernelFn fn, int wpc_even) {
 //    4 workers + courier (160 threads, up to three per SM) instead of 128 CTAs of 8 + 1.
 //  * otherwise: 64-thread single-warp CTAs over as many waves as it takes.
 // DYN, NZ and the control modes run in the single-warp shape with the grid-wide wait only; the kernel comes from the
-// select_step_kernel of the handle's dynamics sampler, control mode and dynamics path.  Host logic only; the CUDA calls are the occupancy
+// select_step_kernel of the handle's control mode and dynamics path.  Host logic only; the CUDA calls are the occupancy
 // queries of a handle's first hand-over and courier decisions, whose errors it returns.
 static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const int NP = h->NP, sms = h->sms;
@@ -551,8 +554,8 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const bool scn = p.use_obst ? ticked_obst
                                 : ((p.scenario >= QS_SCENARIO_DEVICE_FAMILY_FIRST && p.scenario <= QS_SCENARIO_MIX) ||
                                    p.scenario == QS_SCENARIO_EP_RAND_BEZIER || p.scenario == QS_SCENARIO_RUN_AWAY);
-    // qs_set_dynamics_sampler, qs_set_control, qs_set_numpy_dynamics
-    const auto select = select_step_kernel_of[h->dyn_spec != nullptr ? 1 : 0][ctl][h->numpy_dyn ? 1 : 0];
+    // qs_set_control, qs_set_numpy_dynamics
+    const auto select = select_step_kernel_of[ctl][h->numpy_dyn ? 1 : 0];
     auto kernel = [&](bool ho, bool k_dyn, bool k_nz) { return (KernelFn)select(NP, s.split, scn, ho, k_dyn, k_nz); };
     // A balanced grid that will carry the courier warp (the hand-over is, or will be, chosen below): its worker warps per CTA
     // come from the kernel's occupancy (courier_workers), and the env -> block mapping follows them.
@@ -647,12 +650,12 @@ static int launch_step(QsHandle* h, const StepParams& p_in, cudaStream_t s, bool
     h->launches += 1;
     h->started = true;
     note_async(h, s, true);
-    if (h->dyn_every > 0) return launch_dyn_pregen(h, s, nullptr, false);    // the rows this grid's resets did not find
+    if (h->dyn_every > 0) return launch_dyn_pregen(h, s, nullptr, false);    // the rows of the episodes this grid started
     return QS_OK;
 }
 
-// The dynamics sampler's rows ahead of the resets (qs_dyn_pregen_kernel); env_mask != null: before an explicit reset of
-// those envs.
+// The dynamics sampler (qs_dyn_pregen_kernel): ahead, the rows of the envs' next episodes; behind, the live rows of the
+// episodes the step or reset kernel just started (env_mask: that of the reset).
 static int launch_dyn_pregen(QsHandle* h, cudaStream_t s, const uint8_t* env_mask, bool ahead) {
     StepParams p;
     fill_params(h, p);
@@ -1118,7 +1121,7 @@ extern "C" int qs_set_dynamics_sampler(QsHandle* h, const QsDynSampler* spec_hos
     DynSampler* spec = nullptr;
     QS_CUDA(dev_alloc(h, &d0, sizeof(float) * QS_DYN_ROW * A));
     QS_CUDA(dev_alloc(h, &d1, sizeof(float) * QS_DYN_ROW * A));
-    QS_CUDA(dev_alloc(h, &pend, sizeof(int) * E));
+    QS_CUDA(dev_alloc(h, &pend, sizeof(int) * 2 * E));     // [2][E]: row 1 is qs_dyn_pregen_kernel's record
     QS_CUDA(dev_alloc(h, &spec, sizeof(DynSampler)));
     DynSampler ds;
     memset(&ds, 0, sizeof(ds));
@@ -1270,9 +1273,8 @@ extern "C" int qs_reset(QsHandle* h, const uint8_t* env_mask_dev, float* obs_dev
     fill_params(h, p);
     p.obs = obs_dev;
     p.env_mask = env_mask_dev;
-    int rc = QS_OK;
-    if (h->dyn_spec != nullptr) rc = launch_dyn_pregen(h, (cudaStream_t)stream, env_mask_dev, true);      // the rows this reset latches
-    if (rc == QS_OK) rc = launch_reset(h, p, (cudaStream_t)stream);
+    int rc = launch_reset(h, p, (cudaStream_t)stream);
+    if (rc == QS_OK && h->dyn_every > 0) rc = launch_dyn_pregen(h, (cudaStream_t)stream, env_mask_dev, false);     // the rows of the episodes it started
     if (rc == QS_OK && h->pregen_every > 0) rc = launch_pregen(h, (cudaStream_t)stream);
     return rc;
 }
@@ -1301,7 +1303,7 @@ extern "C" int qs_rollout(QsHandle* h, int num_steps, const float* actions_dev, 
     p.obs = obs_dev; p.rewards = rewards_dev; p.dones = dones_dev; p.rew_terms = nullptr;
     p.T = num_steps; p.last_obs_only = last_obs_only ? 1 : 0;
     if (h->dyn_spec == nullptr) return launch_step(h, p, (cudaStream_t)stream);
-    // dynamics sampler: one grid per control step (a row a reset did not find prepared is sampled behind the grid)
+    // dynamics sampler: one grid per control step (the rows of the episodes a grid started are latched behind it)
     const long long A = h->A;
     p.T = 1;
     for (int t = 0; t < num_steps; ++t) {

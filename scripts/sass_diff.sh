@@ -6,7 +6,8 @@
 # Checks out each revision with `git worktree` into a temporary directory, compiles the library's translation units with
 # that revision's NVCC_FLAGS / SRCS (__graft_entry__.py), and prints per kernel whether the SASS is identical once the
 # address and encoding comments are stripped, plus every difference in registers / stack / shared / local memory
-# (cuobjdump --dump-resource-usage).  Exit status 0: every function is identical in both; 1: something differs.
+# (cuobjdump --dump-resource-usage).  Units are matched by file name; the functions of a unit that only one revision has
+# are listed as "only in a" / "only in b".  Exit status 0: every function is identical in both; 1: something differs.
 set -euo pipefail
 
 if [ $# -ne 2 ]; then
@@ -114,14 +115,22 @@ def demangle(names):
     return dict(zip(names, lines))
 
 
+def load(tag, obj, parse, ext):
+    """parse(the unit's dump), or {} where revision `tag` has no such unit"""
+    path = os.path.join(out, tag, obj + ext)
+    return parse(path) if os.path.exists(path) else {}
+
+
+objs = {t: {f for f in os.listdir(os.path.join(out, t)) if f.endswith('.o')} for t in 'ab'}
 differ = 0
-for obj in sorted(f for f in os.listdir(os.path.join(out, 'a')) if f.endswith('.o')):
-    sa, sb = (sass(os.path.join(out, t, obj + '.sass')) for t in 'ab')
-    ra, rb = (resources(os.path.join(out, t, obj + '.res')) for t in 'ab')
+for obj in sorted(objs['a'] | objs['b']):
+    sa, sb = (load(t, obj, sass, '.sass') for t in 'ab')
+    ra, rb = (load(t, obj, resources, '.res') for t in 'ab')
     names = sorted(set(sa) | set(sb))
     pretty = demangle(names)
     same = 0
-    print(f'== {obj[:-2]}: {len(names)} functions')
+    only = '' if obj in objs['a'] and obj in objs['b'] else f' (unit only in {"a" if obj in objs["a"] else "b"})'
+    print(f'== {obj[:-2]}: {len(names)} functions{only}')
     for n in names:
         if n not in sa or n not in sb:
             print(f'  only in {"b" if n in sb else "a"}: {pretty[n]}')
