@@ -177,6 +177,19 @@ int qs_set_reward_coeffs(QsHandle* h, const float* coeffs_host);
 int qs_set_next_episode(QsHandle* h, const uint8_t* env_mask_dev, const float* goals_dev, const float* spawn_dev,
                         const float* obst_xy_dev, void* stream);
 
+/* Pillar radius of the next episode of each env on a host-table handle — the obst_size of
+ * QuadrotorEnvMulti.reset(obst_density, obst_size) (quadrotor_multi.py:339-351; obstacles.py:9-10: radius = size / 2).
+ * radius_dev [E] floats, env_mask_dev [E] bytes or NULL (= all).  Same contract as qs_set_next_episode: each masked env's
+ * next (auto-)reset latches its value, which then sets the collision test, the contact response and the 3x3 distance
+ * patch of that episode; it persists until overwritten.  The first call switches the handle to per-episode radii: every
+ * env's running episode keeps the construction radius (QsConfig.obst_size / 2), and so does every later episode of an env
+ * the calls never mask.  From then on the handle steps without the split step shape, like qs_set_obstacle_randomization.
+ * qs_get_state / qs_set_state carry the running episode's radius (scenario state, scn_f[0].x).  Copies the radii to the
+ * host and synchronises `stream` to check them: every one of the E values must be finite and >= 0.  Fails with
+ * QS_ERR_INVALID_ARG without use_obstacles, or on a handle with a device-side scenario (which draws its sizes with
+ * qs_set_obstacle_randomization). */
+int qs_set_next_obstacle_radius(QsHandle* h, const uint8_t* env_mask_dev, const float* radius_dev, void* stream);
+
 /* replaces `env.goal = ...` assignments made by scenario.step() (e.g. scenarios/swarm_vs_swarm.py:84-85). */
 int qs_set_goals(QsHandle* h, const uint8_t* env_mask_dev, const float* goals_dev, void* stream);
 

@@ -122,6 +122,7 @@ EXPORTS = {
     'qs_ep_len': (C.c_int, [C.c_void_p]),
     'qs_set_reward_coeffs': (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
     'qs_set_next_episode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'qs_set_next_obstacle_radius': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_set_goals': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_reset': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'qs_step': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -432,6 +432,11 @@ __device__ __forceinline__ void reset_env(const StepParams& p, const RngKey& key
             V3 spawn;
             spawn.x = sp.w != 0.f ? sp.x : gq.x; spawn.y = sp.w != 0.f ? sp.y : gq.y; spawn.z = sp.w != 0.f ? sp.z : gq.z;
             rp = reset_pose(episode_key(p, env, g), i, spawn, p.use_obst ? 0.1f : 2.0f);
+            if (p.obst_random) {        // the pillar radius of this episode (qs_set_next_obstacle_radius)
+                const float4 nr = QS_LD(st.next_scn_f + 3 * (long long)env);
+                obst_r = nr.x;
+                if (i == 0) st.scn_f[3 * (long long)env] = nr;
+            }
         }
         if (i == 0) st.epi[env] = make_int2(g, ep.y);
         apply_reset(s, rp);

@@ -33,6 +33,7 @@ struct QsHandle {
     int handover;         // -1 not decided yet, 0 grid-wide wait between step grids, 1 per-block hand-over (plan_step; QS_PDL)
     int courier_wpc;      // 0 not decided yet, else worker warps per CTA of a grid with the courier warp (courier_workers)
     int obst_random, n_obst_counts, n_obst_radii;
+    int obst_r_tables;    // qs_set_next_obstacle_radius was called: a host-table handle with a pillar radius per episode
     int obst_counts[QS_MAX_OBST_CHOICES];
     float obst_radii[QS_MAX_OBST_CHOICES];
     bool wrap_on;
@@ -179,7 +180,8 @@ static void fill_params(const QsHandle* h, StepParams& p) {
     p.obs_stage = (D <= 72) ? 1 : 0;
     p.obs_bulk = 0;
     p.chained = 0;
-    p.obst_random = h->obst_random; p.n_obst_counts = h->n_obst_counts; p.n_obst_radii = h->n_obst_radii;
+    // a per-episode radius from the host (qs_set_next_obstacle_radius) is read where the device-drawn one is
+    p.obst_random = h->obst_random | h->obst_r_tables; p.n_obst_counts = h->n_obst_counts; p.n_obst_radii = h->n_obst_radii;
     for (int k = 0; k < QS_MAX_OBST_CHOICES; ++k) { p.obst_counts[k] = h->obst_counts[k]; p.obst_radii[k] = h->obst_radii[k]; }
     p.scenario = c.scenario; p.grid_l = c.obst_grid[0]; p.grid_w = c.obst_grid[1];
     p.nz = h->nz;
@@ -288,6 +290,21 @@ __global__ void k_set_next_episode(DevState st, int E, int N, int M, const uint8
         const int env = (int)(t / M);
         if (mask == nullptr || mask[env]) st.next_obst[t] = make_float2(obst[2 * t], obst[2 * t + 1]);
     }
+}
+
+// qs_set_next_obstacle_radius: radius[env] -> the next-episode record (next_scn_f[3 env].x, unused by host tables
+// otherwise); the env's next (auto-)reset latches it into scn_f[3 env].x (reset_env).  first: the handle switches to
+// per-episode radii now, so every env's running and next episode get the construction radius first.
+__global__ void k_set_next_obstacle_radius(DevState st, int E, const uint8_t* mask, const float* radius, float init_r, int first) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= E) return;
+    if (first) {
+        float4 f = st.scn_f[3 * t];
+        f.x = init_r;
+        st.scn_f[3 * t] = f;
+        st.next_scn_f[3 * t] = make_float4(init_r, 0.f, 0.f, 0.f);
+    }
+    if (mask == nullptr || mask[t]) st.next_scn_f[3 * t] = make_float4(radius[t], 0.f, 0.f, 0.f);
 }
 
 __global__ void k_set_goals(DevState st, int E, int N, const uint8_t* mask, const float* goals) {
@@ -548,7 +565,7 @@ static int plan_step(QsHandle* h, const StepParams& p, StepShape& s) {
     const bool courier_fits = balance_fits && (wpc + 1) * 32 <= QS_LB;
     const bool courier_shape = h->chained && !grid_wait_only && courier_fits;
     const bool want_split = h->split_mode == 1 || (h->split_mode == -1 && phys_warps <= 4LL * sms && !courier_shape);
-    s.split = want_split && p.obs_stage && NP > 1 && !grid_wait_only && !h->obst_random;
+    s.split = want_split && p.obs_stage && NP > 1 && !grid_wait_only && !p.obst_random;
     const bool balanced = !s.split && balance_fits;
     const bool ticked_obst = p.scenario >= QS_SCENARIO_O_DYNAMIC_SAME_GOAL && p.scenario <= QS_SCENARIO_O_EP_RAND_BEZIER;
     const bool scn = p.use_obst ? ticked_obst
@@ -1259,6 +1276,26 @@ extern "C" int qs_set_next_episode(QsHandle* h, const uint8_t* env_mask_dev, con
     if (obst_xy_dev && !h->cfg.use_obstacles) return fail(QS_ERR_INVALID_ARG, "obstacle table given but use_obstacles = 0");
     return launch_table(h, stream, agents_or_pillars(h), k_set_next_episode, h->st, h->cfg.num_envs, h->cfg.num_agents, h->M,
                         env_mask_dev, goals_dev, spawn_dev, obst_xy_dev);
+}
+
+extern "C" int qs_set_next_obstacle_radius(QsHandle* h, const uint8_t* env_mask_dev, const float* radius_dev, void* stream) {
+    if (!h || !radius_dev) return fail(QS_ERR_INVALID_ARG, "null argument");
+    if (!h->cfg.use_obstacles || h->cfg.scenario != QS_SCENARIO_HOST_TABLES)
+        return fail(QS_ERR_INVALID_ARG, "a per-episode pillar radius from the host needs use_obstacles and host tables "
+                                        "(device-side obstacle scenarios: qs_set_obstacle_randomization)");
+    const int E = h->cfg.num_envs;
+    std::vector<float> r(E);
+    QS_CUDA(cudaSetDevice(h->device));
+    QS_CUDA(cudaMemcpyAsync(r.data(), radius_dev, sizeof(float) * E, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    QS_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+    for (int e = 0; e < E; ++e)
+        if (!(r[e] >= 0.f) || !std::isfinite(r[e])) return fail(QS_ERR_INVALID_ARG, "pillar radii must be finite and >= 0");
+    StepParams p;
+    fill_params(h, p);
+    const int first = h->obst_r_tables ? 0 : 1;
+    const int rc = launch_table(h, stream, E, k_set_next_obstacle_radius, h->st, E, env_mask_dev, radius_dev, p.obst_radius, first);
+    if (rc == QS_OK) h->obst_r_tables = 1;
+    return rc;
 }
 
 extern "C" int qs_set_goals(QsHandle* h, const uint8_t* env_mask_dev, const float* goals_dev, void* stream) {

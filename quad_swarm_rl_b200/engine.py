@@ -189,6 +189,16 @@ class QuadSwarmEngine:
         m = self._dev_mask(env_mask)
         L.check(self.lib.qs_set_next_episode(self.h, _ptr(m), _ptr(g), _ptr(s), _ptr(o), self._stream()))
 
+    def set_next_obstacle_radius(self, radius, env_mask=None):
+        """Pillar radius [E] (size / 2) of each masked env's next episode on a host-table handle (include/quadswarm.h,
+        qs_set_next_obstacle_radius): latched by the env's next (auto-)reset like the tables of set_next_episode, and kept
+        by its later episodes until it changes.  The first call switches the handle to per-episode radii; every env keeps
+        the construction radius until a radius of its own is latched.  A state taken with get_state() before that call
+        holds radius 0 for its running episode."""
+        r = self._dev_f32(radius, (self.E,))
+        m = self._dev_mask(env_mask)
+        L.check(self.lib.qs_set_next_obstacle_radius(self.h, _ptr(m), _ptr(r), self._stream()))
+
     def set_goals(self, goals, env_mask=None):
         g = self._dev_f32(goals, (self.E, self.N, 3))
         m = self._dev_mask(env_mask)

@@ -105,6 +105,8 @@ class _EnvBase:
         self.use_downwash = bool(use_downwash)
         self.use_replay_buffer = use_replay_buffer
         self.obst_density, self.obst_size, self.obst_spawn_area = obst_density, obst_size, obst_spawn_area
+        self._obst_size0 = obst_size                        # the size of the engine's construction radius
+        self._pushed_obst_size = None                       # the size last sent with set_next_obstacle_radius, None: never
         self.ep_time = ep_time
         self.control_freq = 100.0                           # sim_freq / sim_steps, quadrotor_single.py:160
         self.control_dt = 1.0 / self.control_freq
@@ -237,6 +239,18 @@ class _EnvBase:
     def _push_next(self, mask=None):
         self.engine.set_next_episode(self._next['goals'], self._next['spawn'],
                                      self._next['obst'][:, :self.num_obstacles] if self.use_obstacles else None, env_mask=mask)
+
+    def _push_obst_size(self, force=False):
+        """self.obst_size for every episode that starts from now on (engine.set_next_obstacle_radius, radius = size / 2 as
+        obstacles.py:9-10).  Unless forced, a handle that never leaves its construction size is never switched to
+        per-episode radii."""
+        if not self.use_obstacles:
+            return
+        if not force and (self._pushed_obst_size == self.obst_size or
+                          (self._pushed_obst_size is None and self.obst_size == self._obst_size0)):
+            return
+        self.engine.set_next_obstacle_radius(np.full(self.num_envs, self.obst_size / 2.0, np.float32))
+        self._pushed_obst_size = self.obst_size
 
     def can_drones_fly(self):
         """quadrotor_multi.py:281-287: fewer than one floor crash per episode on average over >= 10 episodes."""
@@ -397,8 +411,9 @@ class QuadrotorEnvMulti(_EnvBase):
             if int(obst_density * self.obst_spawn_area[0] * self.obst_spawn_area[1]) > self.num_obstacles:
                 raise NotImplementedError("obst_density above the construction-time density needs a larger pillar table")
             self.obst_density = obst_density
-        if obst_size and obst_size != self.obst_size:
-            raise NotImplementedError("per-episode obstacle size is not supported (SURVEY.md §8f-2)")
+        if obst_size:                            # kept for the later episodes too, as the reference's self.obst_size
+            self.obst_size = obst_size
+        self._push_obst_size()
         obs = self._reset_all()
         return obs[0].cpu().numpy().astype(np.float64)
 
@@ -441,7 +456,8 @@ class QuadrotorEnvMulti(_EnvBase):
         return dict(device={k: (v.clone() if v is not None else None) for k, v in st.items()},
                     scenarios=copy.deepcopy((self._scenarios, self._next_scenarios)), tick=self._tick.copy(),
                     goals=self._goals.copy(), next={k: v.copy() for k, v in self._next.items()},
-                    obst_density=self.obst_density, saved_in_replay_buffer=True,
+                    obst_density=self.obst_density, obst_size=self.obst_size,
+                    obst_size_per_episode=self._pushed_obst_size is not None, saved_in_replay_buffer=True,
                     activate_replay_buffer=self.activate_replay_buffer)
 
     def restore(self, snap, zero_collision_counters=False, keep_rng_counters=True):
@@ -459,6 +475,14 @@ class QuadrotorEnvMulti(_EnvBase):
             live = self.engine.get_state()['env_i32']
             for col in (1, 3, 4 + L.QS_NUM_ENV_STATS + 16):
                 dev['env_i32'][:, col] = live[:, col]
+        # the snapshot's pillar size: that of its running episode travels in the device state (scn_f[0].x), the one of the
+        # episodes after it is set again; a snapshot from before the first size change holds radius 0 there
+        if snap['obst_size_per_episode'] or self._pushed_obst_size is not None:
+            if not snap['obst_size_per_episode']:
+                r0 = np.array([self._obst_size0 / 2.0], np.float32).view(np.int32)[0]
+                dev['env_i32'][:, 4 + L.QS_NUM_ENV_STATS + 4] = int(r0)
+            self.obst_size = snap['obst_size']
+            self._push_obst_size(force=self._pushed_obst_size is None)
         self.engine.set_state(dev)
         self._scenarios, self._next_scenarios = copy.deepcopy(snap['scenarios'])
         for sc in self._scenarios + self._next_scenarios:
